@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py — rows/s of the hot path on B200, next to the HBM roofline and the reference's CPU path.
+"""bench.py — rows/s of the hot path on H100, next to the HBM roofline and the reference's CPU path.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--workload zillow|q6|c1] [--rows R] [--impl reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--workload zillow|q6|c1] [--rows R] [--impl reference] [--dump-outputs DIR]
 
 A "step" is one pass of the stage over the whole synthetic workload. Default workload = BASELINE.json
 configs[1]: the Zillow Z1 pipeline over 100M synthetic rows (cyclic replication of the reference's 32,661-row
@@ -39,9 +39,8 @@ def parse_args():
     ap.add_argument("--cpu-sample-rows", type=int, default=1_000_000)
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--keys", type=int, default=0, help="distinct keys of the aggbykey workload (default rows/100)")
-    ap.add_argument("--min-region-s", type=float, default=2.0,
-                    help="the K-step timed region is repeated (each repeat bracketed by barrier + synchronize) until this much time has "
-                         "been measured; the reported time is the median repeat")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed as DIR/<name>.npy (float32 / float64)")
     ap.add_argument("--no-pageable", action="store_true", help="skip the pageable-host-memory end-to-end variant")
     ap.add_argument("--no-extras", action="store_true", help="default workload only: skip the brief c1 / aggregateByKey measurements")
     return ap.parse_args()
@@ -173,7 +172,7 @@ def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "data sheet (H100 SXM, 3.35 TB/s HBM3)"
 
 
 # ------------------------------------------------------------------------------------------------------
@@ -266,6 +265,66 @@ def build_workload(args):
     blocks = [(pin_cols(W.gen_keyed(total, nkeys, seed=42 + int(os.environ.get("RANK", "0")))), total)]  # every rank its own shard of rows
     return dict(name="aggbykey_str", prog=W.keyed_program(), blocks=blocks, rows=total, in_bytes=total * 20, keep=keep, nkeys=nkeys,
                 desc=f"aggregateByKey string key, {total} rows, {nkeys} distinct keys")
+
+
+DUMP_ROWS = 1 << 16  # rows of a seeded sample when an output has more (keeps a dump of the Zillow columns near 40 MB)
+DUMP_MAX_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, name, prog, results, aggregate=None):
+    """--dump-outputs: what a caller of the timed path receives from its last step, as out_dir/<name>.<field>.npy. A stage's output
+    columns (the blocks' results concatenated in block order; the groups of a hash stage sorted by their key) are sampled to DUMP_ROWS
+    rows by a fixed seed: numeric columns as float64, strings as their UTF-8 bytes (float32) plus per-row lengths (float64), an
+    Option column's validity as float32 0 / 1. An aggregate stage's result (one per block where the caller gets one per block) is
+    float64."""
+    from tuplex_b200 import ir
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {}
+    if aggregate is not None:
+        arrays["aggregate"] = np.array(aggregate, dtype=np.float64).reshape(-1)
+    if results:
+        ncols = len(results[0].out_types())
+        blocks = [r.columns() for r in results]
+        starts = np.cumsum([0] + [len(b[0]) if b else 0 for b in blocks])
+        n = int(starts[-1])
+
+        def values(c, idx):  # values of output column c at global rows idx (bytes for strings), and their validity or None
+            blk = np.searchsorted(starts, idx, side="right") - 1
+            parts = [b[c] for b in blocks]
+            loc = idx - starts[blk]
+            if parts[0].type == ir.T_STR:
+                vals = [bytes(parts[k].data[parts[k].offsets[j]:parts[k].offsets[j + 1]]) for k, j in zip(blk.tolist(), loc.tolist())]
+            else:
+                vals = np.array([parts[k].data[j] for k, j in zip(blk.tolist(), loc.tolist())], dtype=parts[0].data.dtype)
+            valid = None
+            if any(p.valid is not None for p in parts):
+                pres = [np.ones(len(p), bool) if p.valid is None else p.present() for p in parts]
+                valid = np.array([pres[k][j] for k, j in zip(blk.tolist(), loc.tolist())], dtype=bool)
+            return vals, valid
+        order = np.arange(n)
+        if results[0].hash_result and n:  # the table's group order is not defined: sort by the key column
+            key, _ = values(0, order)
+            order = np.array(sorted(range(n), key=lambda i: key[i]), dtype=np.int64) if isinstance(key, list) else np.argsort(key, kind="stable")
+        if n > DUMP_ROWS:
+            order = order[np.sort(np.random.default_rng(0).choice(n, DUMP_ROWS, replace=False))]
+        arrays["rows"] = np.array([n], dtype=np.float64)
+        arrays["sample_rows"] = order.astype(np.float64)
+        names = list(prog.out_names) + [None] * ncols
+        for c in range(ncols):
+            cname = names[c] or f"col{c}"
+            vals, valid = values(c, order)
+            if isinstance(vals, list):
+                arrays[f"{cname}.len"] = np.array([len(v) for v in vals], dtype=np.float64)
+                arrays[f"{cname}.bytes"] = np.frombuffer(b"".join(vals), dtype=np.uint8).astype(np.float32)
+            else:
+                arrays[cname] = vals.astype(np.float64)
+            if valid is not None:
+                arrays[f"{cname}.valid"] = valid.astype(np.float32)
+    total = sum(a.nbytes for a in arrays.values())
+    if total > DUMP_MAX_BYTES:
+        raise RuntimeError(f"--dump-outputs: {total} bytes for {name}, more than {DUMP_MAX_BYTES}")
+    for k, a in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.{k}.npy"), a)
 
 
 # ------------------------------------------------------------------------------------------------------
@@ -440,7 +499,7 @@ def static_config(args, wl_key):
                   "4 columns i64,f64,f64,i64, blocks of 100M rows",
             "c1": "parallelize([1..n]).map(x*x).filter(x%2==0)", "aggbykey": "aggregateByKey string key"}[wl_key]
     return {"workload": WL_NAMES[wl_key], "rows_per_gpu": rows, "description": desc,
-            "l2": "inputs larger than L2 (every block >> 126 MB, distinct HBM buffers per block)"}
+            "l2": "inputs larger than L2 (every block >> 50 MB, distinct HBM buffers per block)"}
 
 
 def reference_line(args):
@@ -518,7 +577,7 @@ def measure_join(args, rank, world, local, dist):
         if dist is not None:
             dist.barrier()
 
-    steps = max(3, min(args.steps, 5))
+    steps = args.steps
     kms, n_out, out_bytes, launches = [], 0, 0, 0
     for _ in range(3):
         jn.probe(pb, ptypes, 0).free()
@@ -577,9 +636,9 @@ def measure_join(args, rank, world, local, dist):
     return out
 
 
-def measure(args, wl_key, rank, world, local, dist, hc):
+def measure(args, wl_key, rank, world, local, dist, hc, dump_dir=None):
     """Device-resident `value`, `roofline`, end-to-end `e2e` (page-locked and pageable host inputs) and the CPU arm of one workload.
-    Returns the fields of its JSON object (rank 0) or None."""
+    Returns the fields of its JSON object (rank 0) or None. dump_dir: where the last timed step's outputs go (--dump-outputs)."""
     import torch
     from tuplex_b200 import backend, ir
     wargs = argparse.Namespace(**vars(args))
@@ -591,7 +650,7 @@ def measure(args, wl_key, rank, world, local, dist, hc):
     if ep == ir.C["TPLX_EP_HASH"]:
         st.hash_reserve(local, wl.get("nkeys", 1 << 20))
 
-    # device-resident copies of every block (distinct HBM: the working set is far larger than the 126 MB L2)
+    # device-resident copies of every block (distinct HBM: the working set is far larger than the 50 MB L2)
     dev_blocks = [backend.Block.upload(local, cols, n) for cols, n in wl["blocks"]]
     torch.cuda.synchronize()
 
@@ -613,11 +672,13 @@ def measure(args, wl_key, rank, world, local, dist, hc):
             tot = ir.bits_f64(st.agg_finish(local, [ir.f64_bits(tot)])[0])
         return tot
 
-    def step_resident():
+    def step_resident(keep=False):
+        """keep: the step's results stay on the device in stats["results"] (fetched after the timed region by --dump-outputs)"""
         kms = 0.0
         launches = 0
         n_out = 0
         partials = []
+        kept = []
         if ep == ir.C["TPLX_EP_HASH"]:
             st.hash_reset(local)
             st.hash_reserve(local, wl.get("nkeys", 1 << 20))
@@ -626,21 +687,25 @@ def measure(args, wl_key, rank, world, local, dist, hc):
             r = st.run(b, 0)   # every block is its own task (row numbers per task), so blocks need not run in sequence
             inf = r.info
             out = (inf.kernel_ms, inf.kernel_launches, int(inf.n_out_rows),
-                   ir.bits_f64(r.aggregate_bits()[0]) if ep == ir.C["TPLX_EP_AGGREGATE"] else None, int(inf.specialised_launches))
-            r.free()
+                   ir.bits_f64(r.aggregate_bits()[0]) if ep == ir.C["TPLX_EP_AGGREGATE"] else None, int(inf.specialised_launches),
+                   r if keep and ep == ir.C["TPLX_EP_MEMORY"] else None)
+            if out[-1] is None:
+                r.free()
             return out
         # row stages: blocks in flight on the GPU's execution lanes (the latency-bound dense launch of one block overlaps the
         # prefilter of the next). Aggregate scans are DRAM-bound (nothing to overlap) and hash stages share one table per
         # device: those run one block at a time.
         runner = pool.map if ep == ir.C["TPLX_EP_MEMORY"] else map
         spec = 0
-        for km, kl, no, part, sl in runner(one_resident, dev_blocks):
+        for km, kl, no, part, sl, res in runner(one_resident, dev_blocks):
             kms += km
             launches += kl
             spec += sl
             n_out += no
             if part is not None:
                 partials.append(part)
+            if res is not None:
+                kept.append(res)
         if ep == ir.C["TPLX_EP_AGGREGATE"]:
             stats["result"] = combine_partials(partials)
         if ep == ir.C["TPLX_EP_HASH"]:
@@ -650,8 +715,11 @@ def measure(args, wl_key, rank, world, local, dist, hc):
             n_out = int(fin.info.n_out_rows)
             kms += fin.info.kernel_ms
             launches += fin.info.kernel_launches
-            fin.free()
-        stats.update(kernel_ms=kms, launches=launches, n_out=n_out, specialised=spec)
+            if keep:
+                kept.append(fin)
+            else:
+                fin.free()
+        stats.update(kernel_ms=kms, launches=launches, n_out=n_out, specialised=spec, results=kept)
 
     def step_e2e(blocks):
         d2h = 0
@@ -720,27 +788,22 @@ def measure(args, wl_key, rank, world, local, dist, hc):
         step_resident()
     clocks = Clocks(local)
     clocks.start()
-    # the K-step region is repeated until min_region_s of it has been measured (a 20-step region of this stage is well under
-    # a second); every repeat is K steps between barrier + synchronize, the reported one is the median repeat (max over ranks)
-    reps = []
+    # exactly K timed steps between barrier + synchronize; with --dump-outputs the last one keeps its results on the device
     kms = 0.0
     launches = 0
-    spent = 0.0
-    while True:
-        kacc = lacc = 0
+    done = 0
 
-        def one_step():
-            nonlocal kacc, lacc
-            step_resident()
-            kacc += stats["kernel_ms"]
-            lacc += stats["launches"]
-        dt_r = max_over_ranks(timed(one_step, args.steps))
-        reps.append((dt_r, kacc, lacc))
-        spent += dt_r
-        if spent >= args.min_region_s or len(reps) >= 200:
-            break
-    reps.sort()
-    dt, kms, launches = reps[len(reps) // 2]
+    def one_step():
+        nonlocal kms, launches, done
+        done += 1
+        step_resident(keep=dump_dir is not None and done == args.steps)
+        kms += stats["kernel_ms"]
+        launches += stats["launches"]
+    dt = max_over_ranks(timed(one_step, args.steps))
+    if dump_dir is not None and rank == 0:
+        dump_outputs(dump_dir, wl["name"], prog, stats["results"], stats.get("result"))
+    for r in stats["results"]:
+        r.free()
 
     # end-to-end through the C ABI with host buffers (H2D of inputs + D2H of results inside the timed region), K steps
     step_e2e(wl["blocks"])
@@ -785,8 +848,7 @@ def measure(args, wl_key, rank, world, local, dist, hc):
                                                                     "(NVRTC): fates + counts in pass 1, outputs in pass 2 from L2, nothing staged")
         line = {
             "value": rows_all / (dt / args.steps), "unit": "rows/s", "ms_per_step": ms_step,
-            "timed_region": {"repeats": len(reps), "seconds_measured": spent, "reported": "median repeat of K steps, max over ranks",
-                             "min_ms_per_step": reps[0][0] / args.steps * 1e3, "max_ms_per_step": reps[-1][0] / args.steps * 1e3},
+            "timed_region": {"steps": args.steps, "seconds_measured": dt, "reported": "K steps between barrier + synchronize, max over ranks"},
             "checks": {"out_rows_per_gpu": stats.get("n_out"), "blocks": len(dev_blocks)},
             "clocks": clk,
             "e2e": {"value": rows_all / (dt_e2e / args.steps), "unit": "rows/s", "h2d_bytes_per_step": e2e_stats.get("h2d", wl["in_bytes"]),
@@ -863,14 +925,14 @@ def main():
         tdist.init_comm(local)  # this rank's NCCL communicator inside libtplx_gpu.so (id broadcast over the launcher's group)
     hc = host_cores()
     keys = ["zillow", "q6"] if args.workload == "both" else [args.workload]
-    parts = {k: measure(args, k, rank, world, local, dist, hc) for k in keys}
+    parts = {k: measure(args, k, rank, world, local, dist, hc, dump_dir=args.dump_outputs) for k in keys}
     extras = {}
     if args.workload == "both" and not args.no_extras:
         # the other two configurations of BASELINE.json, measured briefly in the same run (device-resident value + roofline + e2e):
         # config 0 (fixed-width map/filter through the vector kernel K1v) and one shard of config 5 (aggregateByKey, string keys;
         # under torchrun every rank aggregates its shard and the tables are exchanged on the device)
         xa = argparse.Namespace(**vars(args))
-        xa.steps, xa.min_region_s, xa.no_pageable, xa.no_cpu_baseline = max(3, min(args.steps, 5)), 0.3, True, True
+        xa.no_pageable, xa.no_cpu_baseline = True, True
         xa.rows = 0
         extras["c1"] = measure(xa, "c1", rank, world, local, dist, hc)
         xb = argparse.Namespace(**vars(xa))
@@ -979,26 +1041,32 @@ def main_csv(args, rank, world, local):
         if dist is not None:
             dist.barrier()
 
-    def run_block(buf, fetch):
+    def run_block(buf, fetch, keep=None):
+        """keep: a list that takes (result, parse) instead of freeing them (--dump-outputs)"""
         p = buf.parse(types, delimiter=delim, header=has_header, lazy=lazy)
         r = st.run(p.block, 0)
         inf, pinf = r.info, p.info
         nb = 0
         if is_agg:
             stats["agg"] = ir.bits_f64(r.aggregate_bits()[0])
+            stats.setdefault("aggs", []).append(stats["agg"])
             nb = 8
         elif fetch:
             for c in r.columns():
                 nb += c.nbytes()
         out = (float(pinf.parse_ms), float(inf.kernel_ms), int(pinf.kernel_launches) + int(inf.kernel_launches), int(inf.n_out_rows),
                int(pinf.n_rows), int(pinf.n_bad), sum(int(x) for x in p.block_bytes()), nb)
-        r.free()
-        p.free()
+        if keep is not None and not is_agg:
+            keep.append((r, p))
+        else:
+            r.free()
+            p.free()
         return out
 
-    def step_resident():
+    def step_resident(keep=None):
         acc = [0.0, 0.0, 0, 0, 0, 0, 0, 0]
-        for o in map(lambda b: run_block(b, False), bufs):
+        stats["aggs"] = []
+        for o in map(lambda b: run_block(b, False, keep), bufs):
             for i, v in enumerate(o):
                 acc[i] += v
         stats.update(parse_ms=acc[0], stage_ms=acc[1], launches=acc[2], n_out=acc[3], rows=acc[4], bad=acc[5], col_bytes=acc[6])
@@ -1025,13 +1093,19 @@ def main_csv(args, rank, world, local):
     t0 = time.perf_counter()
     pms = sms = 0.0
     launches = 0
-    for _ in range(args.steps):
-        step_resident()
+    kept = []
+    for i in range(args.steps):
+        step_resident(kept if args.dump_outputs is not None and i == args.steps - 1 else None)
         pms += stats["parse_ms"]
         sms += stats["stage_ms"]
         launches += stats["launches"]
     sync_all()
     dt = time.perf_counter() - t0
+    if args.dump_outputs is not None and rank == 0:
+        dump_outputs(args.dump_outputs, name, prog, [r for r, _ in kept], stats["aggs"] if is_agg else None)
+    for r, p in kept:
+        r.free()
+        p.free()
     e2e_steps = max(1, min(args.steps, 3))
     step_e2e()
     sync_all()
@@ -1059,7 +1133,7 @@ def main_csv(args, rank, world, local):
                 "vs_baseline": None, "dtype": "u8/i64/f64", "data": "synthetic",
                 "config": {"workload": name, "rows_per_gpu": total, "blocks": n_blocks, "csv_bytes_per_gpu": csv_bytes,
                            "description": desc,
-                           "l2": "inputs larger than L2 (every buffer >> 126 MB, distinct HBM buffers)", "out_rows_per_gpu": stats["n_out"]},
+                           "l2": "inputs larger than L2 (every buffer >> 50 MB, distinct HBM buffers)", "out_rows_per_gpu": stats["n_out"]},
                 "clocks": clk,
                 "e2e": {"value": rows_all / (dt_e2e / e2e_steps), "unit": "rows/s", "h2d_bytes_per_step": csv_bytes,
                         "d2h_bytes_per_step": stats.get("d2h", 0), "steps": e2e_steps,
@@ -1067,9 +1141,7 @@ def main_csv(args, rank, world, local):
                 "gpu_launches": launches,
                 "roofline": {"bound": "hbm", "kernel": "csv_tile_states + csv_row_ends + csv_parse_rows + scans + csv_compact + csv_copy_strings (K6)",
                              "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                             # dram__bytes_read + dram__bytes_write of the six K6 kernels per parse, ncu --set full (profiles/r01_csv_k6.md:
-                             # 5.47 GB for 804.1 MB of text), scaled to this buffer size
-                             "traffic": (5.47e9 / 804.1e6 * int(text.size)) if args.workload == "zillow_csv" else None, "peak_source": peak_src,
+                             "traffic": None, "peak_source": peak_src,
                              "algorithmic_bytes_per_row": alg / total, "kernel_ms_per_launch": parse_ms_step / n_blocks,
                              "kernel_share_of_step": parse_ms_step / ms_step, "stage_ms_per_step": sms / args.steps,
                              "csv_gb_per_s": csv_bytes / (parse_ms_step * 1e-3) / 1e9}}

@@ -1,5 +1,5 @@
 /*
- * tplx_gpu.h — C ABI of libtplx_gpu.so, the B200 executor for Tuplex's normal-case
+ * tplx_gpu.h — C ABI of libtplx_gpu.so, the H100 executor for Tuplex's normal-case
  * TransformStage row pipeline.
  *
  * What this boundary replaces in the reference (paths relative to /root/reference/tuplex/):
@@ -100,7 +100,7 @@ int32_t tplx_gpu_stage_destroy(tplx_stage *stage);
 /* The stage specialiser (csrc/jit.inl) — this library's counterpart of the reference's per-stage code generation + JIT
  * (StageBuilder.cc:602-1143, TransformStage::compile TransformStage.cc:763-914): for a stage that sees large blocks the op program
  * is printed as a straight-line CUDA row function and the library's own kernel source is compiled around it at run time (NVRTC,
- * sm_100a) and launched instead of the interpreting kernel — same parameters, same tiles / scans / exception records.
+ * sm_90a) and launched instead of the interpreting kernel — same parameters, same tiles / scans / exception records.
  * Controlled by TPLX_JIT (0 off, 1 = stages with blocks of >= TPLX_JIT_MIN_ROWS rows [default], 2 = always); when NVRTC is not
  * installed the interpreting kernels run. This entry point is the diagnostic view of it and needs no device: the generated row
  * function of `kind` (1 = K1 rows, 2 / 3 = K1v with 8 / 4 rows per thread, 4 = K3 aggregate, 5 = K1m mask) as text,

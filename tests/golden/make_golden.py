@@ -80,3 +80,22 @@ def zillow_reference_udfs():
 
 
 zillow_reference_udfs()
+
+
+def csvmonkey_cells():
+    """tests/golden/csvmonkey_cells.json = digests of the cell dumps of the reference's own csvmonkey reader (oracle/_ref/csv_ref)
+    on the Zillow fixture file and on the seeded inputs with pathological quoting that
+    tests/test_csv_oracle.py::test_cells_equal_reference_csvmonkey generates, ten inputs per digest, in its order."""
+    import json
+    sys.path.insert(0, ROOT)
+    sys.path.insert(0, os.path.dirname(HERE))
+    from oracle import pyoracle as po
+    from test_csv_oracle import cell_digest, csvmonkey_inputs
+    data = gzip.open(os.path.join(HERE, "zillow_noexc.csv.gz"), "rb").read()
+    cases = [po.csv_ref_cells(s) for s, _ in csvmonkey_inputs()]
+    doc = {"zillow": cell_digest([po.csv_ref_cells(data)]), "per_10_inputs": [cell_digest(cases[i:i + 10]) for i in range(0, len(cases), 10)]}
+    with open(os.path.join(HERE, "csvmonkey_cells.json"), "w") as fp:
+        json.dump(doc, fp, indent=0)
+
+
+csvmonkey_cells()

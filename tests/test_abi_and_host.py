@@ -1,4 +1,4 @@
-"""No-GPU checks: the C-ABI library builds for sm_100a, loads, and exports every symbol include/tplx_gpu.h
+"""No-GPU checks: the C-ABI library builds for sm_90a, loads, and exports every symbol include/tplx_gpu.h
 declares; compute entry points fail loudly without a device (no CPU fallback); host-side logic."""
 import ctypes as ct
 import os
@@ -25,10 +25,10 @@ def test_library_exports_every_declared_symbol(built):
     assert sorted(backend.lib()._declared) == declared  # the Python binding covers the whole ABI
 
 
-def test_sass_is_sm100a(built):
+def test_sass_is_sm90a(built):
     import subprocess
     out = subprocess.run(["cuobjdump", "-lelf", os.path.join(ROOT, "tuplex_b200", "lib", "libtplx_gpu.so")], capture_output=True, text=True).stdout
-    assert "sm_100a" in out
+    assert "sm_90a" in out
 
 
 def test_no_cpu_fallback(built):

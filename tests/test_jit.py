@@ -2,7 +2,7 @@
 kernel source compiled around it with NVRTC — this library's counterpart of the reference's per-stage code generation
 (core/src/physical/StageBuilder.cc:602-1143, TransformStage::compile).
 
-CPU part (no GPU): the generated text is what the program says and NVRTC turns it into an sm_100a cubin for hand-written,
+CPU part (no GPU): the generated text is what the program says and NVRTC turns it into an sm_90a cubin for hand-written,
 workload and random programs. GPU part: with TPLX_JIT=2 (every stage specialised at its first block) results are bit-identical to
 the oracle and to the interpreting kernels (TPLX_JIT=0), and the result reports that specialised kernels really ran."""
 import hashlib

@@ -18,7 +18,7 @@ timeout 900 python bench.py > $O/r02_bench_default.json 2> $O/r02_bench_default.
 tail -c 600 $O/r02_bench_default.json
 # launch list of the same command (short: 2 steps, no CPU arms); per-launch times are serialised / cold-cache
 timeout 600 ncu --metrics gpu__time_duration.sum --clock-control none -c 600 --csv --log-file $O/r02_launches.csv \
-  python bench.py --steps 2 --warmup 1 --no-cpu-baseline --no-pageable --no-extras --min-region-s 0 > $O/r02_launches_bench.log 2>&1
+  python bench.py --steps 2 --warmup 1 --no-cpu-baseline --no-pageable --no-extras > $O/r02_launches_bench.log 2>&1
 # one full capture per flagship kernel
 export PROBE_CYCLES=${PROBE_CYCLES:-400}
 [ "${SKIP_OLD:-0}" = "1" ] || timeout 300 ncu --set full --clock-control none --import-source on -k regex:stage_mask -s 3 -c 1 -f -o $O/r02_scan python tools/kernel_probe.py > $O/ncu_a.log 2>&1
@@ -29,5 +29,5 @@ ls -la $O/*.ncu-rep
 # K8: every kernel of one probe of the bench's join workload (count, scan, emit, gathers)
 timeout 200 python tools/join_probe.py > $O/r02_join_probe.log 2>&1
 PROBE_REPEAT=1 timeout 300 ncu --set full --clock-control none --import-source on -k regex:join_ -c 14 -f -o $O/r02_join python tools/join_probe.py > $O/ncu_e.log 2>&1
-[ "${SKIP_OLD:-0}" = "1" ] || timeout 300 ncu --set full --clock-control none --import-source on -k regex:fused_scan_agg_tma -s 1 -c 1 -f -o $O/r02_q6 python bench.py --workload q6 --rows 100000000 --steps 1 --warmup 1 --no-cpu-baseline --no-pageable --min-region-s 0 > $O/ncu_d.log 2>&1
+[ "${SKIP_OLD:-0}" = "1" ] || timeout 300 ncu --set full --clock-control none --import-source on -k regex:fused_scan_agg_tma -s 1 -c 1 -f -o $O/r02_q6 python bench.py --workload q6 --rows 100000000 --steps 1 --warmup 1 --no-cpu-baseline --no-pageable > $O/ncu_d.log 2>&1
 ls -la $O/*.ncu-rep

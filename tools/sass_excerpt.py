@@ -19,7 +19,7 @@ for line in out.splitlines():
 PAT = [("UBLKCP", r"UBLKCP"), ("SYNCS (mbarrier)", r"SYNCS"), ("LDG.E.128", r"LDG\.E\.128"), ("LDG.E.64", r"LDG\.E\.64"), ("LD.E (generic)", r"\bLD\.E"),
        ("LDS.128", r"LDS\.128"), ("STS.128", r"STS\.128"), ("LDS.64", r"LDS\.64"), ("STG.E.64", r"STG\.E\.64"), ("VOTE", r"VOTE"), ("ATOMG/RED", r"ATOMG|RED\.")]
 want = [k for k in data if any(s in k for s in ("stage_mask", "stage_rows", "fused_scan_agg", "stage_hash", "mask_expand", "csv_parse_rows", "join_", "merge_", "valid_"))]
-print("# SASS evidence (cuobjdump -sass tuplex_b200/lib/libtplx_gpu.so, sm_100a)\n")
+print("# SASS evidence (cuobjdump -sass tuplex_b200/lib/libtplx_gpu.so, sm_90a)\n")
 print("| kernel | instructions | " + " | ".join(p[0] for p in PAT) + " |")
 print("|---|---|" + "---|" * len(PAT))
 for k in want:

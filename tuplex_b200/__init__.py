@@ -1,8 +1,8 @@
-"""tuplex_b200 — a B200-native executor for Tuplex's normal-case row pipeline.
+"""tuplex_b200 — an H100-native executor for Tuplex's normal-case row pipeline.
 
 Drop-in surface: `Context.parallelize/csv -> map/filter/withColumn/mapColumn/selectColumns ->
 aggregate/aggregateByKey -> collect` (tuplex/python/tuplex/{context,dataset}.py), executed by hand-written
-sm_100a CUDA kernels behind the C ABI in include/tplx_gpu.h. See DESIGN.md.
+sm_90a CUDA kernels behind the C ABI in include/tplx_gpu.h. See DESIGN.md.
 """
 from .context import Context  # noqa: F401
 from .dataset import DataSet  # noqa: F401

@@ -199,7 +199,7 @@ TPLX_HD void csv_trim_g(G &&get, uint32_t len, uint32_t *pi, uint32_t *pe) {
 }
 
 // A cell of at most 32 bytes in four registers: five independent aligned loads instead of one dependent byte load per
-// character (csv_parse_rows was latency-bound on those, profiles/r01_csv_k6.md).
+// character (csv_parse_rows is latency-bound on those).
 struct CsvCell32 {
     uint64_t w0, w1, w2, w3;
     TPLX_HD void load(const uint8_t *buf, uint32_t b) {

@@ -11,7 +11,7 @@
 // Output row order is therefore: probe rows in input order, matches of one probe row in build-row order. It is part of
 // the contract (tuplex/test/core/JoinTest.cc:135-170) and is what the kernels below produce, deterministically.
 //
-// B200 design. The reference serialises each build row into a malloc'd, realloc-grown bucket; here the build side stays
+// Device design. The reference serialises each build row into a malloc'd, realloc-grown bucket; here the build side stays
 // columnar and the table holds only row numbers:
 //   slots[cap]      open addressing, value = representative build row + 1 of the key that owns the slot (0 = empty). Keys are
 //                   compared against the immutable build key column, so claiming a slot is ONE atomicCAS and needs no
@@ -263,8 +263,8 @@ __global__ void __launch_bounds__(JOIN_NT) join_str_len_kernel(const uint32_t *_
 __global__ void __launch_bounds__(JOIN_NT) join_str_copy_kernel(const uint8_t *__restrict__ src, const uint32_t *__restrict__ src_off,
                                                                 const uint32_t *__restrict__ idx, uint64_t n, const uint64_t *__restrict__ pos,
                                                                 uint32_t *__restrict__ dst_off, uint8_t *__restrict__ dst) {
-    // JOIN_STR_LANES lanes per output row: the strings of this path are short (codes, names: 8 B in the bench's table), a whole warp per
-    // row spent 3.1 G warp-instructions on 45 M rows (ncu, profiles/r02_ncu_kernels.md); 8 lanes keep one byte per lane and row in flight
+    // JOIN_STR_LANES lanes per output row: the strings of this path are short (codes, names: 8 B in the bench's table), so a whole
+    // warp per row would leave most lanes idle; 8 lanes keep one byte per lane and row in flight
     const uint64_t t = (uint64_t)blockIdx.x * JOIN_NT + threadIdx.x;
     const uint64_t i = t / JOIN_STR_LANES;
     const uint32_t sub = (uint32_t)(t % JOIN_STR_LANES);

@@ -1,4 +1,4 @@
-// kernels.cuh — stage kernels for sm_100a.
+// kernels.cuh — stage kernels for sm_90a.
 //
 // K1  stage_rows_kernel   : fused map/filter/withColumn/project over a column block, stable
 //                           compaction (warp ballot bitmaps) + single-pass decoupled look-back scan

@@ -7,7 +7,7 @@
 // here the leading operators up to the selective filter run over every row and only the survivors reach the dense
 // launch (kernels.cuh) that evaluates the whole stage and writes rows.
 //
-// Execution model (B200): every WARP is autonomous. It owns warp-tiles of 32*MR consecutive rows (tile t -> warp
+// Execution model: every WARP is autonomous. It owns warp-tiles of 32*MR consecutive rows (tile t -> warp
 // t mod #warps), a private 2-deep shared-memory ring, and one mbarrier per ring slot. For tile k+1 the lanes
 // 0..n_staged-1 each bring one string column's byte range [offsets[r0], offsets[r1]) and its offsets into the ring
 // with cp.async.bulk (TMA bulk copy, SASS UBLKCP; completion counted on the mbarrier), while the warp evaluates

@@ -118,9 +118,8 @@ extern "C" int32_t tplx_gpu_init(const int32_t *devices, int32_t n) {
         CU(cudaFuncSetAttribute(stage_mask_kernel<true, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, d->smem_optin));
         CU(cudaFuncSetAttribute(stage_mask_kernel<true, 5>, cudaFuncAttributeMaxDynamicSharedMemorySize, d->smem_optin));
         CU(cudaFuncSetAttribute(stage_mask_kernel<true, 6>, cudaFuncAttributeMaxDynamicSharedMemorySize, d->smem_optin));
-        // extra execution lanes on the same GPU (chain d -> alt -> alt ...): TPLX_LANES lanes in all. Measured on the
-        // Zillow bench: 2 lanes 6.18 G rows/s resident / 653 M rows/s end to end; 3 lanes 6.28 G / 625 M; 4 lanes as 3.
-        // The end-to-end number is the headline, so the default stays 2.
+        // extra execution lanes on the same GPU (chain d -> alt -> alt ...): TPLX_LANES lanes in all. Two lanes let the
+        // latency-bound dense launch of one block overlap the prefilter of the next; the default is 2.
         int lanes = 2;
         if (const char *e = getenv("TPLX_LANES")) lanes = std::max(1, std::min(8, atoi(e)));
         Device *tail = d;
@@ -704,7 +703,7 @@ static std::shared_ptr<jit::Binary> jit_binary(tplx_stage *s, int kind, int minb
     else bin->worker = std::thread(jit_compile_job, bin, std::move(src), kind, minb, s->instrs.size());
     return bin;
 }
-// resident CTAs per SM the specialised kernel's register allocation must allow (measured on B200, profiles/r02_jit.md)
+// resident CTAs per SM the specialised kernel's register allocation must allow (TPLX_JIT_MINB* override them)
 static int jit_minb(const tplx_stage *s, int kind) {
     auto env = [](const char *n, int dflt) { const char *e = getenv(n); return e && atoi(e) > 0 ? atoi(e) : dflt; };
     switch (kind) {
@@ -1619,8 +1618,8 @@ static int32_t run_rows(tplx_stage *s, StageDev *sd, const tplx_block *b, int64_
     else CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, stage_rows_kernel, NT, L.total));
     if (occ < 1) return fail(TPLX_E_UNSUPPORTED, "stage kernel cannot be resident");
     // String stages read their input bytes through L1 again and again (every string op walks the bytes): shared memory must not
-    // take the whole 256 KB of the SM. Measured on the Zillow dense launch (B200): 3 CTAs/SM + 60 KB L1 0.413 ms, 4 CTAs/SM + 28 KB L1
-    // 0.54 ms, 2 CTAs/SM + 124 KB L1 0.53 ms. So the carve-out is capped at 196 KB (85 % of 228) and occupancy counted against it.
+    // take the whole 256 KB of the SM's L1 / shared memory. The carve-out is capped at 196 KB (85 % of 228), which leaves 60 KB of
+    // L1 at 3 CTAs/SM, and occupancy is counted against it (TPLX_DENSE_CARVEOUT overrides the cap).
     int carve = s->has_str ? 85 : -1;
     if (getenv("TPLX_DENSE_CARVEOUT")) carve = atoi(getenv("TPLX_DENSE_CARVEOUT"));
     if (jf) jit::cudrv_api()->FuncSetAttribute(jf->fn, jit::CU_FUNC_ATTRIBUTE_PREFERRED_SHARED_MEMORY_CARVEOUT, carve);
@@ -1640,8 +1639,8 @@ static int32_t run_rows(tplx_stage *s, StageDev *sd, const tplx_block *b, int64_
     if (jf) {
         P.n_instr = 0;
         P.n_slots = (uint32_t)s->jit_live.slots.size();
-        // dense-launch prefetch (jit_prefetch): measured on the Zillow dense launch it doubles the DRAM reads (whole 128-byte lines for
-        // cells that need one or two sectors: 433 vs 226 MB per block) and costs 6 %: off unless TPLX_JIT_PREFETCH=1
+        // dense-launch prefetch (jit_prefetch): on the Zillow dense launch it fetches whole 128-byte lines for cells that need one
+        // or two sectors, about twice the DRAM reads: off unless TPLX_JIT_PREFETCH=1
         P.pad_split = (getenv("TPLX_JIT_PREFETCH") && atoi(getenv("TPLX_JIT_PREFETCH"))) ? 0u : 1u;
     }
     if (cols_override)
@@ -1810,8 +1809,8 @@ static int32_t run_mask(tplx_stage *ps, StageDev *psd, const tplx_block *b, tplx
     P.cpool = psd->cpool;
     for (size_t c = 0; c < b->cols.size(); ++c) P.in[c] = b->cols[c];
     // TPLX_MASK_STAGE=1: the string columns the program loads are staged through the warps' shared-memory rings (TMA bulk copies).
-    // Measured on B200 (profiles/r02_zillow.md): the kernel is issue-bound, not latency-bound — staging raises issue utilisation
-    // (62 % -> 71 %) but its per-tile bookkeeping adds 27 % instructions, so plain coalesced loads through L1 are the default.
+    // The kernel is issue-bound rather than latency-bound: staging raises issue utilisation but its per-tile bookkeeping adds
+    // instructions, so plain coalesced loads through L1 are the default.
     const bool want_stage = getenv("TPLX_MASK_STAGE") && atoi(getenv("TPLX_MASK_STAGE")) != 0;
     std::vector<uint32_t> cand;
     for (uint32_t i = 0; i < ps->instrs.size() && want_stage; ++i) {

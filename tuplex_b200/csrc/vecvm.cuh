@@ -4,7 +4,7 @@
 //
 // Same op program, same per-row semantics as vm.cuh (every op is the same single integer / IEEE operation), evaluated
 // VECTOR-AT-A-TIME: a thread owns V = 2J rows of a tile; one instruction dispatch (uniform fetch + jump table) is followed by 2J
-// row operations, so the interpretive overhead per row shrinks by 2J. B200 mapping:
+// row operations, so the interpretive overhead per row shrinks by 2J. Mapping onto the SM:
 //   * inputs: coalesced 128-bit global loads (LDG.E.128: thread t reads rows 2t, 2t+1 of every 512-row slab of the tile);
 //   * ACCUMULATOR CHAINS: the host's vector planner (vec_plan in tplx_gpu.cu) finds the straight-line producer -> consumer pairs of
 //     the program; the consumer takes the value from the thread's registers (the accumulator = result of the previous micro-op)
@@ -310,7 +310,7 @@ struct VecVM {
 // ---- tile tail: ranks by the owner, block-wide decoupled look-back, dense write (fixed-width outputs only) ---------------------
 // The scalar kernel's look-back (rows_tile_finish: one warp, a 32-tile window per round, K values behind a status flag and a fence)
 // is fine for heavy tiles; a fixed-width tile is evaluated in ~1-2 us, and then the speed at which inclusive prefixes propagate
-// (32 tiles per L2 round trip) bounds the whole kernel (measured: 59 G rows/s on C1). Here a tile's scan state is ONE 64-bit word
+// (32 tiles per L2 round trip) bounds the whole kernel. Here a tile's scan state is ONE 64-bit word
 //   [status:2 | rows kept:31 | exception rows:31]   status 1 = this tile's counts, 2 = inclusive prefix
 // written with a single relaxed store (no fence: status and values travel together), and ALL 256 threads look back at once: thread t
 // polls tile - 1 - t, the block adds the counts up to the nearest inclusive word — 256 tiles per round trip.
@@ -416,9 +416,9 @@ __device__ __forceinline__ void jit_eval_vec(const ulonglong2 (&vin)[J][JIT_NIN]
 
 #if defined(TPLX_JIT) && (TPLX_JIT_KIND == 6 || TPLX_JIT_KIND == 7)
 // ---- K1w: the specialised fixed-width row kernel with WIDE tiles ---------------------------------------------------------------------
-// Measured on C1 (profiles/r02_jit.md): with the interpretation gone, K1v is bound by the latency chain of a tile — ticket, LDG,
+// On C1, with the interpretation gone, K1v is bound by the latency chain of a tile — ticket, LDG,
 // counts, look-back over every earlier tile still in flight, stores — of which the look-back waits for the SLOWEST load among all
-// predecessors (in-order retirement over a window of ~1000 tiles): ~10-14 us per 2048-row tile however few instructions the tile takes.
+// predecessors (in-order retirement over a window of ~1000 tiles), however few instructions the tile takes.
 // Only resident warps hide that, and a specialised row function leaves registers and shared memory to spare. So a CTA takes B = 4 (or 2)
 // sub-batches of 2048 rows per ticket: one ticket, one count barrier, ONE look-back and one inclusive-prefix publication per 8192 rows,
 // 64 KB of loads per CTA between two waits; the sub-batches are evaluated back to back (the LDG.128s of sub-batch b + 1 are issued before
@@ -616,15 +616,14 @@ extern "C" __global__ void __launch_bounds__(NT, TPLX_JIT_MINB) tplx_jit_kernel(
 
 #if defined(TPLX_JIT) && (TPLX_JIT_KIND >= 8 && TPLX_JIT_KIND <= 11)
 // ---- K1r: the specialised fixed-width row kernel that stages NOTHING: L2 is the staging buffer ----------------------------------------
-// Per-tile phase clocks of K1w on C1 (tools/tile_times.py, profiles/r02_jit.md): load + evaluate 5.4 us, counts 1.0 us, look-back 5.5 us
-// (= waiting for the slowest load among the ~1000 tiles in flight: in-order retirement), stores 3.0 us. Rows sit in shared memory from
-// their evaluation to their store, ~12 us, and shared memory bounds the rows in flight (148 x 227 KB / 8 B = 4 M rows): throughput =
-// rows in flight / latency = what was measured. Short of making DRAM latency deterministic, the way out is to hold rows in flight
-// somewhere bigger: the 126 MB L2. K1r evaluates a tile TWICE:
+// Per-tile phase clocks of K1w on C1 (tools/tile_times.py): load + evaluate, counts, look-back (= waiting for the slowest load among the
+// ~1000 tiles in flight: in-order retirement), stores. Rows sit in shared memory from their evaluation to their store, and shared memory
+// bounds the rows in flight (132 SMs x 227 KB / 8 B = 3.8 M rows on H100): throughput = rows in flight / latency. Short of making DRAM
+// latency deterministic, the way out is to hold rows in flight somewhere bigger: the 50 MB L2. K1r evaluates a tile TWICE:
 //   pass 1: LDG.128 the inputs, run the row function for the row's FATE only (kept / filtered / raised: two bits per row in registers),
 //           count, publish — nothing is staged;
-//   pass 2: once the tile's offset is known, LDG.128 the same inputs again (read a few microseconds ago: L2 hits, ncu: DRAM reads
-//           1.15 x algorithmic), run the row function again and store the outputs of the kept rows straight from registers.
+//   pass 2: once the tile's offset is known, LDG.128 the same inputs again (read a few microseconds ago: L2 hits), run the row
+//           function again and store the outputs of the kept rows straight from registers.
 // DRAM traffic stays algorithmic (one read, one write), the second read costs L2 bandwidth and the second evaluation instructions — a
 // trade for programs of a few operations (the planner picks K1r for those, K1w otherwise). No shared memory beyond the counts, so a
 // CTA can keep TWO tiles in flight for the price of ten registers: the look-back of tile A (the wait for the slowest of its predecessors)
@@ -835,8 +834,8 @@ __global__ void __launch_bounds__(NT, 4) stage_rows_vec_kernel(const __grid_cons
     const uint32_t lt = (1u << lane) - 1u;
 
     // Tickets are taken when the tile starts, not ahead of time: a ticket held while its owner still works on the previous tile
-    // stalls the look-back of every later tile (measured: 103 -> 77 G rows/s on C1 with one ticket of lookahead; loading the next
-    // tile's input under the look-back of this one: 149 -> 112 G rows/s). Thread 0 takes the next ticket when IT has finished the
+    // stalls the look-back of every later tile (so does loading the next tile's input under the look-back of this one: both were slower
+    // on C1). Thread 0 takes the next ticket when IT has finished the
     // tile (its atomic overlaps the other warps' stores) and one barrier at the top of the loop publishes it.
     if (tid == 0) s_ctl[0] = atomicAdd(&P.counters[0], 1u);
     while (true) {

@@ -1,4 +1,4 @@
-// vm.cuh — per-row evaluator of the tplx op program on sm_100a.
+// vm.cuh — per-row evaluator of the tplx op program on sm_90a.
 //
 // Replaces the body of the LLVM-generated processRow pipeline
 // (reference tuplex/core/src/physical/PipelineBuilder.cc:90-170,565-1025) and the UDF code that
