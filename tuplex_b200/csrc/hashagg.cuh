@@ -190,7 +190,10 @@ __global__ void hash_init_accs(HashTableDev T, uint32_t n_accs, const AccP *accs
 
 // =============================================================================================
 // K4: rows in -> hash table.  Same tile/VM structure as K3; the per-row sink is the table.
+// EXC_ONLY: collect the exception records only and leave the table alone (second pass over a block whose exception rows did
+// not fit the first pass's buffer).
 // =============================================================================================
+template <bool EXC_ONLY>
 __global__ void __launch_bounds__(NT) stage_hash_kernel(const KParams *__restrict__ Pg, const HashParams *__restrict__ Hg) {
     extern __shared__ __align__(16) uint8_t smem[];
     const KParams &P = *Pg;
@@ -210,10 +213,11 @@ __global__ void __launch_bounds__(NT) stage_hash_kernel(const KParams *__restric
         reinterpret_cast<uint4 *>(s_prog)[i] = reinterpret_cast<const uint4 *>(P.prog)[i];
     for (uint32_t i = tid; i < P.n_in * (sizeof(ColIn) / 8); i += NT)
         reinterpret_cast<uint64_t *>(s_cols)[i] = reinterpret_cast<const uint64_t *>(P.in)[i];
-    for (uint32_t i = tid; i < SM_BUCKETS; i += NT) {
-        s_bkey[i] = HT_NOT_FOUND;
-        for (uint32_t k = 0; k < P.n_accs; ++k) s_bacc[(size_t)k * SM_BUCKETS + i] = acc_identity(P.accs[k].kind);
-    }
+    if (!EXC_ONLY)
+        for (uint32_t i = tid; i < SM_BUCKETS; i += NT) {
+            s_bkey[i] = HT_NOT_FOUND;
+            for (uint32_t k = 0; k < P.n_accs; ++k) s_bacc[(size_t)k * SM_BUCKETS + i] = acc_identity(P.accs[k].kind);
+        }
     if (tid < 4) s_stat[tid] = 0;
     __syncthreads();
 
@@ -234,7 +238,7 @@ __global__ void __launch_bounds__(NT) stage_hash_kernel(const KParams *__restric
             t.exc_code = 0;
             t.scr_used = 0;
             VM<NT>::run(s_prog, 0, P.n_instr, s_regs, s_cols, row, row, P.cpool, t);
-            if (t.alive) {
+            if (!EXC_ONLY && t.alive) {
                 uint32_t blob = 0;
                 const uint64_t h = hash_key<NT>(H, s_regs, &blob);
                 const uint32_t g = find_or_insert<NT>(H, s_regs, h, blob);
@@ -298,12 +302,13 @@ __global__ void __launch_bounds__(NT) stage_hash_kernel(const KParams *__restric
         __syncthreads();
     }
     // flush the pre-aggregation buckets
-    for (uint32_t i = tid; i < SM_BUCKETS; i += NT) {
-        const uint32_t g = s_bkey[i];
-        if (g == HT_NOT_FOUND) continue;
-        for (uint32_t k = 0; k < na; ++k)
-            atomic_acc_global(P.accs[k].kind, &H.ht.accs[(size_t)k * H.ht.cap + g], s_bacc[(size_t)k * SM_BUCKETS + i]);
-    }
+    if (!EXC_ONLY)
+        for (uint32_t i = tid; i < SM_BUCKETS; i += NT) {
+            const uint32_t g = s_bkey[i];
+            if (g == HT_NOT_FOUND) continue;
+            for (uint32_t k = 0; k < na; ++k)
+                atomic_acc_global(P.accs[k].kind, &H.ht.accs[(size_t)k * H.ht.cap + g], s_bacc[(size_t)k * SM_BUCKETS + i]);
+        }
 }
 
 // ---- table maintenance ----------------------------------------------------------------------------

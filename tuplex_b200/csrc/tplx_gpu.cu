@@ -113,7 +113,8 @@ extern "C" int32_t tplx_gpu_init(const int32_t *devices, int32_t n) {
         CU(cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &thr));
         CU(cudaFuncSetAttribute(stage_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, d->smem_optin));
         CU(cudaFuncSetAttribute(stage_agg_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, d->smem_optin));
-        CU(cudaFuncSetAttribute(stage_hash_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, d->smem_optin));
+        CU(cudaFuncSetAttribute(stage_hash_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, d->smem_optin));
+        CU(cudaFuncSetAttribute(stage_hash_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, d->smem_optin));
         CU(cudaFuncSetAttribute(stage_mask_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, d->smem_optin));
         CU(cudaFuncSetAttribute(stage_mask_kernel<true, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, d->smem_optin));
         CU(cudaFuncSetAttribute(stage_mask_kernel<true, 5>, cudaFuncAttributeMaxDynamicSharedMemorySize, d->smem_optin));

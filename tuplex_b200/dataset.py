@@ -1012,8 +1012,10 @@ def _acc_combine(kind: int, a, b):
 
 def _py_fold(row_ops, end: Op, value, obj, names, exc_counter):
     try:
-        val, _ = pyexec.run_row(row_ops, obj, names)
-        return end.udf(value, val)
+        val, names2 = pyexec.run_row(row_ops, obj, names)
+        # the aggregate UDF sees the row as on the device path: a Row (columns by name or index), one column as the value itself
+        r = pyexec.Row(val if isinstance(val, tuple) else (val,), names2)
+        return end.udf(value, r if len(r) != 1 else r[0])
     except Dropped:
         return value
     except Exception as ex:  # noqa: BLE001
