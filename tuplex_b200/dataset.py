@@ -11,17 +11,21 @@ them on the CPython path, merge in order.
 """
 from __future__ import annotations
 
-import struct
+import threading
 from collections import Counter
+from concurrent.futures import ThreadPoolExecutor
 from typing import Any, Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
 
 from . import backend, ir, pyexec
 from .backend import Column
-from .frontend import StageCompiler, UnsupportedUDF
+from .frontend import StageCompiler, UnsupportedUDF, Val
 from .ir import C, T_BOOL, T_F64, T_I64, T_STR
 from .pyexec import Dropped, Op
+
+_ENDPOINTS = ("aggregate", "aggregateByKey", "unique")  # operators that end a stage
+_metrics_lock = threading.Lock()  # ctx.metrics is updated from one thread per device
 
 
 def _clone_op(op: Op) -> Op:
@@ -205,12 +209,8 @@ class DataSet:
         (fast_csvwriter, PipelineBuilder.cc:1550-1722): on the device (K7, tplx_gpu_result_csv) when the last stage ran
         there without rows from the interpreter path, else by the host twin `_csv_cell`."""
         import os
-        self._csv_sink = []
-        try:
-            rows, names = self._execute(sink="csv")
-            chunks = self._csv_sink
-        finally:
-            self._csv_sink = None
+        chunks: List[bytes] = []
+        rows, names = self._execute(csv_sink=chunks)
         os.makedirs(path, exist_ok=True) if not path.endswith(".csv") else None
         fn = path if path.endswith(".csv") else os.path.join(path, "part0.csv")
         with open(fn, "wb") as fp:
@@ -238,22 +238,7 @@ class DataSet:
         py = {T_I64: int, T_F64: float, T_BOOL: bool, T_STR: str}
         if self._join is None and self._parent is None and self._source is not None and not hasattr(self._source, "chunks"):
             try:
-                sc = StageCompiler([c.type for c in self._source.cols], self._source.names, _option_cols(self._source.cols))
-                for o in self._ops:
-                    if o.kind == "map":
-                        sc.add_map(o.udf, o.id)
-                    elif o.kind == "filter":
-                        sc.add_filter(o.udf, o.id)
-                    elif o.kind == "withColumn":
-                        sc.add_with_column(o.column, o.udf, o.id)
-                    elif o.kind == "mapColumn":
-                        sc.add_map_column(o.column, o.udf, o.id)
-                    elif o.kind == "selectColumns":
-                        sc.add_select(o.columns, o.id)
-                    elif o.kind == "renameColumn":
-                        sc.add_rename(o.column, o.extra, o.id)
-                    else:
-                        raise UnsupportedUDF("endpoint")
+                sc = _compile_row_ops(self._source, self._ops)
                 return [typing.Optional[py[v.type]] if v.null is not None else py[v.type] for v in sc.row]
             except (UnsupportedUDF, KeyError):
                 pass
@@ -307,30 +292,14 @@ class DataSet:
         fall back to reading the UDF's return expression."""
         if self._parent is None and self._source is not None and len(self._source.cols) == len(names):
             try:
-                sc = StageCompiler([c.type for c in self._source.cols], self._source.names, _option_cols(self._source.cols))
-                for o in self._ops:
-                    if o.kind == "map":
-                        sc.add_map(o.udf, o.id)
-                    elif o.kind == "filter":
-                        sc.add_filter(o.udf, o.id)
-                    elif o.kind == "withColumn":
-                        sc.add_with_column(o.column, o.udf, o.id)
-                    elif o.kind == "mapColumn":
-                        sc.add_map_column(o.column, o.udf, o.id)
-                    elif o.kind == "selectColumns":
-                        sc.add_select(o.columns, o.id)
-                    elif o.kind == "renameColumn":
-                        sc.add_rename(o.column, o.extra, o.id)
-                    else:
-                        break
-                    if o is op:
-                        return list(sc.names)
+                return list(_compile_row_ops(self._source, self._ops[:self._ops.index(op) + 1]).names)
             except Exception:  # noqa: BLE001 — UnsupportedUDF or a UDF the front end cannot read
                 pass
         return _map_output_names(op.udf, names)
 
-    def _execute(self, dry: bool = False, sink: Optional[str] = None):
-        """Split the operator chain into stages and run them. Returns (python rows, column names)."""
+    def _execute(self, csv_sink: Optional[list] = None):
+        """Split the operator chain into stages and run them. Returns (python rows, column names). With `csv_sink` (a list) the
+        last stage may instead write its rows there as CSV text and return (None, column names)."""
         src = self._source
         self._last_exceptions = Counter()
         if self._join is not None:
@@ -344,7 +313,7 @@ class DataSet:
         stages: List[List[Op]] = [[]]
         for op in self._ops:
             stages[-1].append(op)
-            if op.kind in ("aggregate", "aggregateByKey", "unique"):
+            if op.kind in _ENDPOINTS:
                 stages.append([])
         if not stages[-1] and len(stages) > 1:
             stages.pop()
@@ -353,8 +322,7 @@ class DataSet:
             if si > 0:
                 src = self._ctx._source_from_rows(rows, names)
             last = si == len(stages) - 1
-            rows, names = _run_stage(self._ctx, src, ops, self._last_exceptions,
-                                     csv_sink=self._csv_sink if (sink == "csv" and last) else None)
+            rows, names = _run_stage(self._ctx, src, ops, self._last_exceptions, csv_sink=csv_sink if last else None)
         return rows, names
 
 
@@ -415,6 +383,43 @@ def _option_cols(cols) -> List[int]:
     return [c for c, col in enumerate(cols) if getattr(col, "valid", None) is not None]
 
 
+def _compile_row_ops(src: Source, ops: Sequence[Op]) -> StageCompiler:
+    """A stage compiler over `src`'s columns fed the row operators `ops`; UnsupportedUDF for a UDF outside the GPU op set and
+    for any operator that is not a row operator."""
+    sc = StageCompiler([c.type for c in src.cols], src.names, _option_cols(src.cols))
+    for op in ops:
+        if op.kind == "map":
+            sc.add_map(op.udf, op.id)
+        elif op.kind == "filter":
+            sc.add_filter(op.udf, op.id)
+        elif op.kind == "withColumn":
+            sc.add_with_column(op.column, op.udf, op.id)
+        elif op.kind == "mapColumn":
+            sc.add_map_column(op.column, op.udf, op.id)
+        elif op.kind == "selectColumns":
+            sc.add_select(op.columns, op.id)
+        elif op.kind == "renameColumn":
+            sc.add_rename(op.column, op.extra, op.id)
+        else:
+            raise UnsupportedUDF(f"{op.kind} is not a row operator")
+    return sc
+
+
+def _per_device(devs: List[int], blocks: list, fn) -> list:
+    """fn(device, its blocks) for every device, each over a contiguous share of `blocks`, so that concatenating the results in
+    device order keeps block order. Several devices run on one thread each, all at once (their collectives meet); the results
+    come back in device order and the first error is re-raised."""
+    from .dist import shard_range
+
+    def task(k: int):
+        lo, hi = shard_range(len(blocks), k, len(devs))
+        return fn(devs[k], blocks[lo:hi])
+    if len(devs) == 1:
+        return [task(0)]
+    with ThreadPoolExecutor(len(devs)) as ex:
+        return list(ex.map(task, range(len(devs))))
+
+
 def _rows_as_tuples(rows):
     return [r if isinstance(r, tuple) else (r,) for r in rows]
 
@@ -464,59 +469,35 @@ def _run_join(ctx, spec: JoinSpec, exc_counter: Counter):
         rcols.append(Column(T_I64, rsrc.orig_index if rsrc.orig_index is not None else np.arange(rsrc.n_rows, dtype=np.int64)))
     probe_cols, build_cols, pk, bk = (lcols, rcols, li, ri) if build_right else (rcols, lcols, ri, li)
     n_probe, n_build = (lsrc.n_rows, rsrc.n_rows) if build_right else (rsrc.n_rows, lsrc.n_rows)
-    devs = list(getattr(ctx, "_devices", [ctx._device])) or [ctx._device]
     block_rows = ctx._block_rows
     blocks = [(lo, min(n_probe, lo + block_rows)) for lo in range(0, n_probe, block_rows)] or [(0, 0)]
-    if len(blocks) < 2:
-        devs = devs[:1]  # a single probe block has nothing to shard
+    devs = ctx._devices if len(blocks) > 1 else [ctx._device]  # a single probe block has nothing to shard
     backend.init(sorted(set(devs)))
-    from .dist import shard_range
-    import threading
-    mlock = threading.Lock()
 
-    def run_shard(k: int):
+    def run_shard(dev: int, dev_blocks):
         """One task per device: the table is built once per device (broadcast of the small side), the device's contiguous run of
         probe blocks goes through it in order; no exchange between devices."""
-        dev = devs[k]
         bb = backend.Block.upload(dev, build_cols, n_build)
         jn = backend.Join(bb, [c.type for c in build_cols], bk)
         outs = []
-        blo, bhi = shard_range(len(blocks), k, len(devs))
-        for lo, hi in blocks[blo:bhi]:
+        for lo, hi in dev_blocks:
             cols = [c.slice(lo, hi) for c in probe_cols] if (lo, hi) != (0, n_probe) else probe_cols
             pb = backend.Block.upload(dev, cols, hi - lo)
             res = jn.probe(pb, [c.type for c in probe_cols], pk, left_outer=left_outer, build_first=not build_right)
             info = res.info
-            with mlock:
+            with _metrics_lock:
                 ctx.metrics._add(info)
                 ctx.metrics.join_probe_rows = getattr(ctx.metrics, "join_probe_rows", 0) + (hi - lo)
             outs.append(res.columns())
             res.free()
             pb.free()
-        with mlock:
+        with _metrics_lock:
             ctx.metrics.join_build_ms = getattr(ctx.metrics, "join_build_ms", 0.0) + jn.info["build_ms"]
         jn.free()
         bb.free()
         return outs
 
-    if len(devs) == 1:
-        shard_outs = [run_shard(0)]
-    else:
-        shard_outs: List[Any] = [None] * len(devs)
-        errs: List[BaseException] = []
-
-        def work(k):
-            try:
-                shard_outs[k] = run_shard(k)
-            except BaseException as e:  # noqa: BLE001
-                errs.append(e)
-        ths = [threading.Thread(target=work, args=(k,)) for k in range(len(devs))]
-        for t in ths:
-            t.start()
-        for t in ths:
-            t.join()
-        if errs:
-            raise errs[0]
+    shard_outs = _per_device(devs, blocks, run_shard)
     col_vals: Optional[List[list]] = None
     for outs in shard_outs:
         for oc in outs:
@@ -533,8 +514,7 @@ def _run_join(ctx, spec: JoinSpec, exc_counter: Counter):
         return rows, names
     # ---- interpreter path for the fallback rows of either side, merged in (probe row, build row) order ----
     # device layout with the index columns: first side's non-key columns (its index last), key, second side's non-key columns (index last)
-    n_first = (n_left_cols if build_right else n_left_cols)  # left columns always come first
-    left_idx_pos = n_first - 1                    # left non-key columns are n_left_cols - 1 payloads + the index column
+    left_idx_pos = n_left_cols - 1  # left columns always come first: n_left_cols - 1 non-key payloads, then the index column
     right_idx_pos = len(col_vals) - 1
     lidx, ridx = col_vals[left_idx_pos], col_vals[right_idx_pos]
     keep = [i for i in range(len(col_vals)) if i not in (left_idx_pos, right_idx_pos)]
@@ -618,305 +598,297 @@ def _py_join_pairs(L, li, R, ri, left_outer, build_right, n_right_cols):
 
 def _run_stage(ctx, src: Source, ops: List[Op], exc_counter: Counter, csv_sink: Optional[list] = None):
     """One TransformStage on the GPU + CPython resolve of its exception rows."""
-    end = ops[-1] if ops and ops[-1].kind in ("aggregate", "aggregateByKey", "unique") else None
+    end = ops[-1] if ops and ops[-1].kind in _ENDPOINTS else None
     row_ops = ops[:-1] if end else ops
-    in_types = [c.type for c in src.cols]
     is_csv = hasattr(src, "chunks")  # csvsource.CsvSource: the device parses the file right in front of the stage
-    if is_csv and not in_types:  # missing / empty file: nothing to run (python/tests/test_csv.py:66-69)
-        return _run_stage_python(ctx, Source([], [], 0, None, [], 0), ops, exc_counter)
-    prog = None
+    if is_csv and not src.cols:  # missing / empty file: nothing to run (python/tests/test_csv.py:66-69)
+        return _run_stage_python(Source([], [], 0, None, [], 0), ops, exc_counter)
     try:
-        sc = StageCompiler(in_types, src.names, _option_cols(src.cols))
-        for op in row_ops:
-            if op.resolvers or op.ignores:
-                pass  # resolvers only act on the slow path
-            if op.kind == "map":
-                sc.add_map(op.udf, op.id)
-            elif op.kind == "filter":
-                sc.add_filter(op.udf, op.id)
-            elif op.kind == "withColumn":
-                sc.add_with_column(op.column, op.udf, op.id)
-            elif op.kind == "mapColumn":
-                sc.add_map_column(op.column, op.udf, op.id)
-            elif op.kind == "selectColumns":
-                sc.add_select(op.columns, op.id)
-            elif op.kind == "renameColumn":
-                sc.add_rename(op.column, op.extra, op.id)
-        out_names = list(sc.names)
-        need_rowidx = end is None and (bool(src.fallback) or is_csv)
-        if end is None:
-            if need_rowidx:
-                sc.begin_op(row_ops[-1].id if row_ops else 0)
-                d = sc.new_vreg(T_I64)
-                sc.emit(C["TPLX_OP_LDROW"], d)
-                from .frontend import Val
-                sc.row.append(Val(T_I64, d))
-                sc.names.append("__rowidx")
-            prog = sc.finish_memory()
-        elif end.kind == "aggregate":
-            prog = sc.finish_aggregate(end.udf, end.extra[0], end.extra[1], end.id)
-        elif end.kind == "aggregateByKey":
-            prog = sc.finish_hash(end.columns, end.udf, end.extra[0], end.extra[1], end.id)
-        else:
-            prog = sc.finish_hash(list(range(len(sc.row))), None, None, None, end.id)
+        plan = _compile_stage(src, row_ops, end)
     except UnsupportedUDF as e:
         ctx._log(f"stage falls back to the CPython path: {e}")
-        return _run_stage_python(ctx, src.to_host_source() if is_csv else src, ops, exc_counter)
+        return _run_stage_python(src.to_host_source() if is_csv else src, ops, exc_counter)
+    backend.init(sorted(set(ctx._devices)))
+    stage = backend.Stage(plan.prog)
+    hold = csv_sink is not None
+    shards = [_csv_blocks(ctx, plan, stage, src, hold)] if is_csv else _column_blocks(ctx, plan, stage, src, hold)
+    st = _stitch(shards, src.fallback)
+    if end is None:
+        rows, names = _rows_endpoint(plan, st, src, exc_counter, csv_sink), plan.out_names
+    elif end.kind == "aggregate":
+        rows, names = _aggregate_endpoint(plan, st, src.names, exc_counter)
+    else:
+        rows, names = _hash_endpoint(plan, stage, st, list(dict.fromkeys(sh.dev for sh in shards)), src.names, exc_counter)
+    stage.close()
+    return rows, names
 
-    used_cols = list(range(len(in_types)))
-    if is_csv:  # projection pushdown: the device decodes only the columns the stage loads
-        used_cols = ir.referenced_inputs(prog)
-        if len(used_cols) > C["TPLX_MAX_COLS"]:
-            ctx._log(f"stage reads {len(used_cols)} columns (> TPLX_MAX_COLS): CPython path")
-            return _run_stage_python(ctx, src.to_host_source(), ops, exc_counter)
-        ir.project_inputs(prog, used_cols)
-    dev = ctx._device
-    backend.init(sorted(set(getattr(ctx, "_devices", [dev]))))
-    stage = backend.Stage(prog)
-    block_rows = ctx._block_rows
-    in_values: Optional[List[list]] = None  # python values of input columns, built lazily for resolve
 
-    csv_rows: Dict[int, Any] = {}  # CSV input: python value of the rows the interpreter path needs
+class _StagePlan:
+    """A stage compiled for the device: its program, the operators it runs and the layout of its columns."""
 
-    def input_row(i: int):
-        nonlocal in_values
-        if is_csv:
-            return csv_rows[i]
-        if in_values is None:
-            in_values = [c.to_values() for c in src.cols]
-        return _row_of(src.cols, in_values, i)
+    def __init__(self, prog, row_ops: List[Op], end: Optional[Op], out_names: List[Optional[str]], need_rowidx: bool,
+                 used_cols: Optional[List[int]]):
+        self.prog, self.row_ops, self.end = prog, row_ops, end
+        self.out_names = out_names      # output column names, without __rowidx
+        self.need_rowidx = need_rowidx  # the last output column (__rowidx) holds each row's input row number
+        self.used_cols = used_cols      # CSV source: the file columns the device decodes
 
-    fallback = list(src.fallback)
-
-    n = src.n_rows
-    starts = list(range(0, n, block_rows)) or [0]
-    devs = list(getattr(ctx, "_devices", [dev])) or [dev]
-    if is_csv or len(starts) < 2:
-        devs = devs[:1]  # the CSV source parses chunk after chunk on one device; a single block has nothing to shard
-    import threading
-    mlock = threading.Lock()
-
-    class Shard:
-        """What one task (= one device's contiguous run of blocks, LocalBackend.cc:679-735) produced."""
-        def __init__(self):
-            self.out_cols: List[List[Column]] = []
-            self.excs: List[np.ndarray] = []
-            self.partials: List[List[int]] = []
-            self.held: List[tuple] = []
-            self.row_no = 0  # rows written + exceptions so far (TransformTask::_outputRowCounter)
-
-    def fetch_cols(res, lo, rowmap):
+    def fetch_cols(self, res, lo: int, rowmap: Optional[np.ndarray]) -> List[Column]:
+        """Output columns of the block whose first data row is input row `lo`, __rowidx turned into input row numbers."""
         oc = res.columns()
-        if need_rowidx:
+        if self.need_rowidx:
             if rowmap is not None:
                 oc[-1].data = rowmap[oc[-1].data]
             oc[-1].data += lo
         return oc
 
-    def consume(sh: "Shard", res, lo, parse, data):
-        """Take one block's result into the shard (exception records, output columns or partial aggregate)."""
+
+def _compile_stage(src: Source, row_ops: List[Op], end: Optional[Op]) -> _StagePlan:
+    """The stage's device program; UnsupportedUDF when it has to run on the CPython path. A row stage over input that has rows
+    the device does not run (fallback rows, bad CSV rows) also outputs the input row number of each row (__rowidx), by which
+    those rows are merged back in. A CSV stage decodes only the file columns the program loads (projection pushdown)."""
+    is_csv = hasattr(src, "chunks")
+    sc = _compile_row_ops(src, row_ops)
+    out_names = list(sc.names)
+    need_rowidx = end is None and (bool(src.fallback) or is_csv)
+    if end is None:
+        if need_rowidx:
+            sc.begin_op(row_ops[-1].id if row_ops else 0)
+            d = sc.new_vreg(T_I64)
+            sc.emit(C["TPLX_OP_LDROW"], d)
+            sc.row.append(Val(T_I64, d))
+            sc.names.append("__rowidx")
+        prog = sc.finish_memory()
+    elif end.kind == "aggregate":
+        prog = sc.finish_aggregate(end.udf, end.extra[0], end.extra[1], end.id)
+    elif end.kind == "aggregateByKey":
+        prog = sc.finish_hash(end.columns, end.udf, end.extra[0], end.extra[1], end.id)
+    else:
+        prog = sc.finish_hash(list(range(len(sc.row))), None, None, None, end.id)
+    used_cols = None
+    if is_csv:
+        used_cols = ir.referenced_inputs(prog)
+        if len(used_cols) > C["TPLX_MAX_COLS"]:
+            raise UnsupportedUDF(f"stage reads {len(used_cols)} columns (> TPLX_MAX_COLS)")
+        ir.project_inputs(prog, used_cols)
+    return _StagePlan(prog, row_ops, end, out_names, need_rowidx, used_cols)
+
+
+class _Shard:
+    """What one task (= one device's contiguous run of blocks, LocalBackend.cc:679-735) produced; after _stitch, the whole stage."""
+
+    def __init__(self, dev: Optional[int]):
+        self.dev = dev
+        self.out_cols: List[List[Column]] = []
+        self.excs: List[np.ndarray] = []          # exception records of each block (input row, row_no, operator id)
+        self.partials: List[List[int]] = []       # partial aggregate of each block
+        self.held: List[tuple] = []               # CSV sink: (result, lo, rowmap, first row_no, device) until the writer is chosen
+        self.fallback: List[Tuple[int, Any]] = []  # (input row, python object) of the rows the device did not run
+        self.inputs: Dict[int, Any] = {}          # input row -> python object, for the rows whose UDF raised on the device
+        self.row_no = 0  # rows written + exceptions so far (TransformTask::_outputRowCounter)
+
+    def take(self, ctx, plan: _StagePlan, res, lo: int, exc: np.ndarray, rowmap: Optional[np.ndarray], hold: bool):
+        """Take one block's result: its exception records (`exc`, rows counted from the block's first data row, input row `lo`),
+        then its output columns, its partial aggregate or, with `hold`, the result itself."""
         info = res.info
-        with mlock:
+        with _metrics_lock:
             ctx.metrics._add(info)
-        exc = res.exceptions()
-        rowmap = None
-        if parse is not None:
-            pinfo = parse.info
-            ctx.metrics.csv_rows += int(pinfo.n_rows)
-            ctx.metrics.csv_bad_rows += int(pinfo.n_bad)
-            ctx.metrics.csv_parse_ms += float(pinfo.parse_ms)
-            if pinfo.n_bad:  # block row -> data row
-                rowmap = parse.rowmap().astype(np.int64)
-                raw = data.tobytes()
-                for bad in parse.bad_rows():
-                    fallback.append((lo + int(bad["row"]), src.line_object(raw[int(bad["line_start"]):int(bad["line_end"])], False)))
         if len(exc):
-            exc = exc.copy()
-            if rowmap is not None:
-                exc["row"] = rowmap[exc["row"]]
-            if parse is not None:  # text of the rows whose UDF raised, decoded as the device decoded them
-                ends = parse.row_ends().astype(np.int64)
-                ends[0] = -1 if ends[0] == 0xFFFFFFFF else ends[0]
-                raw = data.tobytes()
-                for r_ in exc["row"]:
-                    a_ = int(ends[r_]) + 1
-                    while raw[a_] in (10, 13):
-                        a_ += 1
-                    csv_rows[lo + int(r_)] = src.line_object(raw[a_:int(ends[r_ + 1])], True)
             exc["row"] += lo
-            sh.excs.append(exc)
-        if prog.endpoint == C["TPLX_EP_MEMORY"]:
-            frn = sh.row_no  # the block ran with this first_row_no
-            sh.row_no += int(info.n_out_rows) + int(info.n_exceptions)
-            if csv_sink is not None:
-                sh.held.append((res, lo, rowmap, frn, getattr(sh, "dev", dev)))  # decide at the end: device CSV writer or column fetch + merge
+            self.excs.append(exc)
+        if plan.prog.endpoint == C["TPLX_EP_MEMORY"]:
+            first_row_no = self.row_no  # the block ran with this first_row_no
+            self.row_no += int(info.n_out_rows) + int(info.n_exceptions)
+            if hold:
+                self.held.append((res, lo, rowmap, first_row_no, self.dev))
                 return
-            sh.out_cols.append(fetch_cols(res, lo, rowmap))
-        elif prog.endpoint == C["TPLX_EP_AGGREGATE"]:
-            sh.partials.append(res.aggregate_bits())
+            self.out_cols.append(plan.fetch_cols(res, lo, rowmap))
+        elif plan.prog.endpoint == C["TPLX_EP_AGGREGATE"]:
+            self.partials.append(res.aggregate_bits())
         res.free()
 
-    shards: List[Shard] = []
-    agg_combined: Optional[List[int]] = None
-    hash_shares: List[List[Column]] = []
-    if is_csv:
-        sh = Shard()
-        base = 0
-        col_types = [t if c in used_cols else backend.CSV_SKIP for c, t in enumerate(in_types)]
-        lazy = csv_lazy_columns(prog, used_cols, in_types)
-        for data, skip_header in src.chunks():
-            buf = backend.CsvBuffer(dev, data)
-            parse = buf.parse(col_types, src.delimiter, src.quotechar, skip_header, src.null_values, lazy=lazy)
-            consume(sh, stage.run(parse.block, sh.row_no), base, parse, data)
-            base += int(parse.info.n_rows)
-            parse.free()
-            buf.free()
-        src.total_rows = base
-        shards.append(sh)
-    else:
-        # blocks are sharded contiguously over the context's devices (tuplex.gpu.devices): one task per device, its blocks in
-        # order; concatenating the shards in device order preserves the input order (LocalBackend.cc:1104-1152). Map / filter
-        # stages exchange nothing; aggregate endpoints combine through the C ABI's collectives when every device is distinct.
-        from .dist import shard_range
-        blocks = [(lo, min(n, lo + block_rows)) for lo in starts]
-        phys = len(set(devs)) == len(devs) and len(devs) > 1  # distinct physical devices: NCCL communicator over them
-        if phys:
-            ctx._ensure_local_comm(devs)
+    def exceptions(self) -> np.ndarray:
+        return np.concatenate(self.excs) if self.excs else np.zeros(0, dtype=backend.EXC_DTYPE)
 
-        def run_shard(k: int) -> Shard:
-            sh = Shard()
-            sh.dev = devs[k]
-            blo, bhi = shard_range(len(blocks), k, len(devs))
-            for lo, hi in blocks[blo:bhi]:
-                cols = [c.slice(lo, hi) for c in src.cols] if (lo, hi) != (0, n) else src.cols
-                consume(sh, stage.run_host(devs[k], cols, hi - lo, sh.row_no), lo, None, None)
-            if len(devs) > 1 and prog.endpoint == C["TPLX_EP_AGGREGATE"] and phys:
-                # this device's partial = its blocks folded in block order; collective: NCCL all-gather + fold in device order
-                part = None
-                for p in sh.partials:
-                    part = p if part is None else [_acc_bits(a.kind, _acc_combine(a.kind, _acc_value(a.kind, x), _acc_value(a.kind, y)))
-                                                   for a, x, y in zip(prog.accs, part, p)]
-                if part is None:
-                    part = [_acc_identity_bits(a.kind) for a in prog.accs]
-                sh.partials = [stage.agg_finish(devs[k], part)]
-            if len(devs) > 1 and prog.endpoint == C["TPLX_EP_HASH"] and phys:
-                stage.hash_exchange(devs[k])  # collective: afterwards this device's table holds the groups it owns
-            return sh
+    def interpreter_rows(self) -> list:
+        """Python objects of the rows outside the normal case: rows whose UDF raised on the device, then fallback rows."""
+        return [self.inputs[int(e["row"])] for e in self.exceptions()] + [obj for _, obj in self.fallback]
 
-        if len(devs) == 1:
-            shards = [run_shard(0)]
-        else:
-            from concurrent.futures import ThreadPoolExecutor
-            with ThreadPoolExecutor(len(devs)) as ex:
-                shards = list(ex.map(run_shard, range(len(devs))))
-            if prog.endpoint == C["TPLX_EP_AGGREGATE"] and phys:
-                agg_combined = shards[0].partials[0]  # every device holds the same combined bits
-    # one numbering over the whole stage: a shard's row numbers continue where the previous shard stopped
-    out_cols_all: List[List[Column]] = []
-    exc_all: List[np.ndarray] = []
-    agg_partials: List[List[int]] = []
-    held: List[tuple] = []
-    off = 0
+
+def _csv_blocks(ctx, plan: _StagePlan, stage, src, hold: bool) -> _Shard:
+    """The block loop of a CSV source: one device parses chunk after chunk (K6) right in front of the stage. Rows that do not
+    parse become fallback rows; the rows whose UDF raised are decoded from their text as the device decoded them."""
+    sh = _Shard(ctx._device)
+    in_types = [c.type for c in src.cols]
+    col_types = [t if c in plan.used_cols else backend.CSV_SKIP for c, t in enumerate(in_types)]
+    lazy = csv_lazy_columns(plan.prog, plan.used_cols, in_types)
+    base = 0
+    for data, skip_header in src.chunks():
+        buf = backend.CsvBuffer(sh.dev, data)
+        parse = buf.parse(col_types, src.delimiter, src.quotechar, skip_header, src.null_values, lazy=lazy)
+        res = stage.run(parse.block, sh.row_no)
+        pinfo, exc, rowmap = parse.info, res.exceptions(), None
+        ctx.metrics.csv_rows += int(pinfo.n_rows)
+        ctx.metrics.csv_bad_rows += int(pinfo.n_bad)
+        ctx.metrics.csv_parse_ms += float(pinfo.parse_ms)
+        raw = data.tobytes() if (pinfo.n_bad or len(exc)) else b""
+        if pinfo.n_bad:  # block row -> data row
+            rowmap = parse.rowmap().astype(np.int64)
+            for bad in parse.bad_rows():
+                sh.fallback.append((base + int(bad["row"]), src.line_object(raw[int(bad["line_start"]):int(bad["line_end"])], False)))
+        if len(exc):
+            if rowmap is not None:
+                exc["row"] = rowmap[exc["row"]]
+            ends = parse.row_ends().astype(np.int64)
+            ends[0] = -1 if ends[0] == 0xFFFFFFFF else ends[0]
+            for r in exc["row"]:
+                a = int(ends[r]) + 1
+                while raw[a] in (10, 13):
+                    a += 1
+                sh.inputs[base + int(r)] = src.line_object(raw[a:int(ends[r + 1])], True)
+        sh.take(ctx, plan, res, base, exc, rowmap, hold)
+        base += int(pinfo.n_rows)
+        parse.free()
+        buf.free()
+    src.total_rows = base
+    return sh
+
+
+def _column_blocks(ctx, plan: _StagePlan, stage, src: Source, hold: bool) -> List[_Shard]:
+    """The block loop of a column source: blocks are sharded contiguously over the context's devices (tuplex.gpu.devices), one
+    task per device, its blocks in order; concatenating the shards in device order preserves the input order
+    (LocalBackend.cc:1104-1152). Map / filter stages exchange nothing; aggregate endpoints combine through the C ABI's
+    collectives when every device is distinct."""
+    prog, n, block_rows = plan.prog, src.n_rows, ctx._block_rows
+    blocks = [(lo, min(n, lo + block_rows)) for lo in range(0, n, block_rows)] or [(0, 0)]
+    devs = ctx._devices if len(blocks) > 1 else [ctx._device]  # a single block has nothing to shard
+    phys = len(set(devs)) == len(devs) and len(devs) > 1  # distinct physical devices: NCCL communicator over them
+    if phys:
+        ctx._ensure_local_comm(devs)
+
+    def run_shard(dev: int, dev_blocks) -> _Shard:
+        sh = _Shard(dev)
+        for lo, hi in dev_blocks:
+            cols = [c.slice(lo, hi) for c in src.cols] if (lo, hi) != (0, n) else src.cols
+            res = stage.run_host(dev, cols, hi - lo, sh.row_no)
+            sh.take(ctx, plan, res, lo, res.exceptions(), None, hold)
+        if phys and prog.endpoint == C["TPLX_EP_AGGREGATE"]:
+            # this device's partial = its blocks folded in block order; collective: NCCL all-gather + fold in device order
+            part = None
+            for p in sh.partials:
+                part = p if part is None else [_acc_bits(a.kind, _acc_combine(a.kind, _acc_value(a.kind, x), _acc_value(a.kind, y)))
+                                               for a, x, y in zip(prog.accs, part, p)]
+            if part is None:
+                part = [_acc_identity_bits(a.kind) for a in prog.accs]
+            sh.partials = [stage.agg_finish(dev, part)]
+        if phys and prog.endpoint == C["TPLX_EP_HASH"]:
+            stage.hash_exchange(dev)  # collective: afterwards this device's table holds the groups it owns
+        return sh
+
+    shards = _per_device(devs, blocks, run_shard)
+    if phys and prog.endpoint == C["TPLX_EP_AGGREGATE"]:
+        for sh in shards[1:]:
+            sh.partials = []  # every device holds the same combined bits
+    if any(sh.excs for sh in shards):
+        vals = [c.to_values() for c in src.cols]
+        for sh in shards:
+            sh.inputs = {int(i): _row_of(src.cols, vals, int(i)) for e in sh.excs for i in e["row"]}
+    return shards
+
+
+def _stitch(shards: List[_Shard], fallback: List[Tuple[int, Any]]) -> _Shard:
+    """The shards as one record, behind the source's `fallback` rows, with one numbering over the whole stage: a shard's row
+    numbers continue where the previous shard stopped."""
+    st = _Shard(None)
+    st.fallback = list(fallback)
     for sh in shards:
         for e in sh.excs:
-            if off:
-                e["row_no"] += off
-            exc_all.append(e)
-        off += sh.row_no
-        out_cols_all += sh.out_cols
-        agg_partials += sh.partials
-        held += sh.held
-    if agg_combined is not None:
-        agg_partials = [agg_combined]
-    excs = np.concatenate(exc_all) if exc_all else np.zeros(0, dtype=backend.EXC_DTYPE)
+            e["row_no"] += st.row_no
+        st.row_no += sh.row_no
+        st.out_cols += sh.out_cols
+        st.excs += sh.excs
+        st.partials += sh.partials
+        st.held += sh.held
+        st.fallback += sh.fallback
+        st.inputs.update(sh.inputs)
+    return st
 
-    # ---- endpoints --------------------------------------------------------------------------------
-    if prog.endpoint == C["TPLX_EP_MEMORY"]:
-        ncols = len(prog.out_cols) - prog.hidden_out_cols
-        if csv_sink is not None:
-            # CSV sink: when no row took the interpreter path the rows are formatted on the device (K7) in block order
-            ok = not len(excs) and not fallback and not any(prog.out_null_of)  # the device writer prints values, not None cells
-            if ok:
-                for res, *_ in held:
-                    txt = res.csv_bytes(n_cols=ncols - (1 if need_rowidx else 0))
-                    if txt is None:  # f64 output column: host formatter
-                        ok = False
-                        break
-                    csv_sink.append(txt)
-            elif len(excs) and not fallback and not is_csv and not need_rowidx and not any(prog.out_null_of):
-                # exception rows: resolve them in CPython, put the resolved rows back into their slots ON THE DEVICE (K9,
-                # ResolveTask::executeInOrder) and keep the device row writer
-                chunks = _device_merge_csv(held, row_ops, src, input_row, [t for _, t in prog.out_cols[:ncols]], exc_counter)
-                if chunks is not None:
-                    csv_sink.extend(chunks)
-                    ok = True
-            if ok:
-                for res, *_ in held:
-                    res.free()
-                stage.close()
-                return None, out_names
-            del csv_sink[:]
-            for res, lo_, rowmap_, *_ in held:
-                out_cols_all.append(fetch_cols(res, lo_, rowmap_))
+
+def _rows_endpoint(plan: _StagePlan, st: _Shard, src: Source, exc_counter: Counter, csv_sink: Optional[list]):
+    """Memory endpoint: the normal-case rows with the rows resolved on the CPython path merged in, in order. With a CSV sink
+    the device writes the text into `csv_sink` when it can, and None is returned."""
+    prog, row_ops = plan.prog, plan.row_ops
+    ncols = len(prog.out_cols) - prog.hidden_out_cols
+    user_cols = ncols - (1 if plan.need_rowidx else 0)
+    excs = st.exceptions()
+    if csv_sink is not None:
+        # the device row writer (K7) prints values, not None cells. Exception rows resolved in CPython go back into their slots
+        # ON THE DEVICE (K9, ResolveTask::executeInOrder), except when they must merge with fallback rows by __rowidx
+        chunks = None
+        if not st.fallback and not any(prog.out_null_of) and not (len(excs) and plan.need_rowidx):
+            chunks = _device_merge_csv(st.held, row_ops, src.names, st.inputs, [t for _, t in prog.out_cols[:user_cols]], exc_counter)
+        if chunks is not None:
+            csv_sink.extend(chunks)
+            for res, *_ in st.held:
                 res.free()
-        merged_vals = [sum((oc[c].to_values() for oc in out_cols_all), []) for c in range(ncols)]
-        n_out = len(merged_vals[0]) if ncols else 0
-        user_cols = ncols - (1 if need_rowidx else 0)
-        normal_rows = [tuple(merged_vals[c][i] for c in range(user_cols)) if user_cols != 1 else merged_vals[0][i] for i in range(n_out)]
-        # resolve exception rows in CPython, merge by row number (ResolveTask::executeInOrder)
-        resolved: List[Tuple[int, int, Any]] = []  # (input row, row_no, value) for rows that produced output
-        for e in excs:
-            i = int(e["row"])
-            try:
-                val, _ = pyexec.run_row(row_ops, input_row(i), src.names)
-                resolved.append((i, int(e["row_no"]), val))
-            except Dropped:
-                pass
-            except Exception as ex:  # noqa: BLE001 — stays an exception, counted like the reference's exception_counts
-                exc_counter[(getattr(ex, "tplx_op", int(e["op_id"])), type(ex).__name__)] += 1
-        if not need_rowidx:
-            rows = _merge_by_rowno(normal_rows, excs, resolved)
-        else:
-            # rows outside the normal-case schema run entirely on the CPython path; merge by original position
-            idx_normal = merged_vals[-1]
-            orig = src.orig_index
-            keyed = [(int(orig[j]) if orig is not None else int(j), r) for j, r in zip(idx_normal, normal_rows)]
-            keyed += [(int(orig[i]) if orig is not None else i, v) for i, _, v in resolved]
-            for pos, obj in fallback:
-                try:
-                    val, _ = pyexec.run_row(row_ops, obj, src.names)
-                    keyed.append((pos, val))
-                except Dropped:
-                    pass
-                except Exception as ex:  # noqa: BLE001
-                    exc_counter[(getattr(ex, "tplx_op", 0), type(ex).__name__)] += 1
-            keyed.sort(key=lambda t: t[0])
-            rows = [r for _, r in keyed]
-        stage.close()
-        return rows, out_names
+            return None
+        for res, lo, rowmap, *_ in st.held:
+            st.out_cols.append(plan.fetch_cols(res, lo, rowmap))
+            res.free()
+    merged_vals = [sum((oc[c].to_values() for oc in st.out_cols), []) for c in range(ncols)]
+    n_out = len(merged_vals[0]) if ncols else 0
+    normal_rows = [tuple(merged_vals[c][i] for c in range(user_cols)) if user_cols != 1 else merged_vals[0][i] for i in range(n_out)]
+    # resolve exception rows in CPython, merge by row number (ResolveTask::executeInOrder)
+    resolved: List[Tuple[int, int, Any]] = []  # (input row, row_no, value) for rows that produced output
+    for e in excs:
+        r = _run_py(row_ops, st.inputs[int(e["row"])], src.names, exc_counter, int(e["op_id"]))
+        if r is not None:
+            resolved.append((int(e["row"]), int(e["row_no"]), r[0]))
+    if not plan.need_rowidx:
+        return _merge_by_rowno(normal_rows, excs, resolved)
+    # rows outside the normal-case schema run entirely on the CPython path; merge by original position
+    orig = src.orig_index
+    keyed = [(int(orig[j]) if orig is not None else int(j), r) for j, r in zip(merged_vals[-1], normal_rows)]
+    keyed += [(int(orig[i]) if orig is not None else i, v) for i, _, v in resolved]
+    for pos, obj in st.fallback:
+        r = _run_py(row_ops, obj, src.names, exc_counter, 0)
+        if r is not None:
+            keyed.append((pos, r[0]))
+    keyed.sort(key=lambda t: t[0])
+    return [r for _, r in keyed]
 
-    if prog.endpoint == C["TPLX_EP_AGGREGATE"]:
-        combine, init = end.extra
-        inits = list(init) if isinstance(init, (tuple, list)) else [init]
-        # thread slot starts from the initial value; partials combined in block (partition) order
-        # (TransformTask.cc:218-230,278-299)
-        accs = list(inits)
-        for part in agg_partials:
-            vals = [_acc_value(a.kind, b) for a, b in zip(prog.accs, part)]
-            accs = [_acc_combine(a.kind, x, y) for a, x, y in zip(prog.accs, accs, vals)]
-        value = tuple(accs) if isinstance(init, (tuple, list)) else accs[0]
-        # exception rows + fallback rows: fold on the CPython path with the user's own aggregate UDF
-        for i in [int(e["row"]) for e in excs]:
-            value = _py_fold(row_ops, end, value, input_row(i), src.names, exc_counter)
-        for _, obj in fallback:
-            value = _py_fold(row_ops, end, value, obj, src.names, exc_counter)
-        stage.close()
-        return [value], [None] * (len(value) if isinstance(value, tuple) else 1)
 
-    # hash endpoint: every distinct device holds the groups it owns after the exchange (a single table otherwise)
+def _aggregate_endpoint(plan: _StagePlan, st: _Shard, names, exc_counter: Counter):
+    """Aggregate endpoint: the thread slot starts from the initial value and takes the partials in block (partition) order
+    (TransformTask.cc:218-230,278-299); exception rows and fallback rows are then folded in on the CPython path with the user's
+    own aggregate UDF."""
+    prog, end = plan.prog, plan.end
+    init = end.extra[1]
+    accs = list(init) if isinstance(init, (tuple, list)) else [init]
+    for part in st.partials:
+        vals = [_acc_value(a.kind, b) for a, b in zip(prog.accs, part)]
+        accs = [_acc_combine(a.kind, x, y) for a, x, y in zip(prog.accs, accs, vals)]
+    value = tuple(accs) if isinstance(init, (tuple, list)) else accs[0]
+    for obj in st.interpreter_rows():
+        r = _run_py(plan.row_ops, obj, names, exc_counter, end.id)
+        if r is None:
+            continue
+        try:
+            value = end.udf(value, _endpoint_arg(*r))
+        except Exception as ex:  # noqa: BLE001
+            exc_counter[(end.id, type(ex).__name__)] += 1
+    return [value], [None] * (len(value) if isinstance(value, tuple) else 1)
+
+
+def _hash_endpoint(plan: _StagePlan, stage, st: _Shard, devs: List[int], names, exc_counter: Counter):
+    """Hash endpoint (aggregateByKey, unique): each of `devs` holds the groups it owns after the exchange (a single table
+    otherwise). Rows outside the normal case (other types, CSV rows with nulls / unparsable cells, rows whose UDF raised on
+    the device) are resolved by the interpreter and join the groups like any other row (ResolveTask feeds the same hash sink,
+    core/src/physical/ResolveTask.cc:618-700)."""
+    prog, end = plan.prog, plan.end
     nk = prog.n_keys
     vals: List[list] = []
-    for dv in (sorted(set(devs), key=devs.index) if not is_csv else [dev]):
+    for dv in devs:
         res = stage.hash_finish(dv)
         cols = res.columns()
         res.free()
@@ -929,51 +901,32 @@ def _run_stage(ctx, src: Source, ops: List[Op], exc_counter: Counter, csv_sink: 
         key = tuple(vals[c][i] for c in range(nk))
         table[key] = [vals[nk + k][i] for k in range(len(prog.accs))]
         order.append(key)
-    if end.kind == "aggregateByKey" and (len(excs) or fallback):
-        combine, init = end.extra
-        pending = [input_row(int(e["row"])) for e in excs] + [obj for _, obj in fallback]
-        for obj in pending:
-            try:
-                val, names2 = pyexec.run_row(row_ops, obj, src.names)
-            except Dropped:
-                continue
-            except Exception as ex:  # noqa: BLE001
-                exc_counter[(getattr(ex, "tplx_op", 0), type(ex).__name__)] += 1
-                continue
-            r = pyexec.Row(val if isinstance(val, tuple) else (val,), names2)
-            key = tuple(r[k] for k in end.columns)
-            cur = table.get(key)
-            cur_v = (tuple(cur) if isinstance(init, (tuple, list)) else cur[0]) if cur is not None else init
-            try:
-                nv = end.udf(cur_v, r if len(r) != 1 else r[0])
-            except Exception as ex:  # noqa: BLE001
-                exc_counter[(end.id, type(ex).__name__)] += 1
-                continue
-            if cur is None:
-                order.append(key)
-            table[key] = list(nv) if isinstance(nv, tuple) else [nv]
-    elif end.kind == "unique" and (len(excs) or fallback):
-        # rows outside the normal case (other types, CSV rows with nulls / unparsable cells, rows whose UDF raised on the device)
-        # are resolved by the interpreter and join the set like any other row (ResolveTask feeds the same hash sink,
-        # core/src/physical/ResolveTask.cc:618-700)
-        pending = [input_row(int(e["row"])) for e in excs] + [obj for _, obj in fallback]
-        for obj in pending:
-            try:
-                val, _ = pyexec.run_row(row_ops, obj, src.names)
-            except Dropped:
-                continue
-            except Exception as ex:  # noqa: BLE001
-                exc_counter[(getattr(ex, "tplx_op", 0), type(ex).__name__)] += 1
-                continue
+    init = end.extra[1] if end.kind == "aggregateByKey" else None
+    for obj in st.interpreter_rows():
+        r = _run_py(plan.row_ops, obj, names, exc_counter, 0)
+        if r is None:
+            continue
+        val, row_names = r
+        if end.kind == "unique":
             key = val if isinstance(val, tuple) else (val,)
             if key not in table:
                 table[key] = []
                 order.append(key)
+            continue
+        key = _group_key(val, row_names, end.columns)
+        cur = table.get(key)
+        cur_v = (tuple(cur) if isinstance(init, (tuple, list)) else cur[0]) if cur is not None else init
+        try:
+            nv = end.udf(cur_v, _endpoint_arg(val, row_names))
+        except Exception as ex:  # noqa: BLE001
+            exc_counter[(end.id, type(ex).__name__)] += 1
+            continue
+        if cur is None:
+            order.append(key)
+        table[key] = list(nv) if isinstance(nv, tuple) else [nv]
     order.sort(key=_key_order)
     rows = [tuple(list(k) + table[k]) if (len(k) + len(table[k])) != 1 else k[0] for k in order]
-    names = list(prog.out_names) + [None] * len(prog.accs)
-    stage.close()
-    return rows, names
+    return rows, list(prog.out_names) + [None] * len(prog.accs)
 
 
 def _acc_value(kind: int, bits: int):
@@ -1010,17 +963,27 @@ def _acc_combine(kind: int, a, b):
     return max(a, b)
 
 
-def _py_fold(row_ops, end: Op, value, obj, names, exc_counter):
+def _run_py(row_ops: Sequence[Op], obj, names, exc_counter: Counter, default_op: int):
+    """One row through `row_ops` on the CPython path: (value, names), or None when the row was dropped or raised. A raise stays an
+    exception, counted like the reference's exception_counts under the operator that raised (`default_op` when not tagged)."""
     try:
-        val, names2 = pyexec.run_row(row_ops, obj, names)
-        # the aggregate UDF sees the row as on the device path: a Row (columns by name or index), one column as the value itself
-        r = pyexec.Row(val if isinstance(val, tuple) else (val,), names2)
-        return end.udf(value, r if len(r) != 1 else r[0])
+        return pyexec.run_row(row_ops, obj, names)
     except Dropped:
-        return value
+        return None
     except Exception as ex:  # noqa: BLE001
-        exc_counter[(getattr(ex, "tplx_op", end.id), type(ex).__name__)] += 1
-        return value
+        exc_counter[(getattr(ex, "tplx_op", default_op), type(ex).__name__)] += 1
+        return None
+
+
+def _endpoint_arg(val, names):
+    """A row as an aggregate UDF sees it, the same on every path: a Row (columns by name or index), one column as the value itself."""
+    r = pyexec.Row(val if isinstance(val, tuple) else (val,), names)
+    return r if len(r) != 1 else r[0]
+
+
+def _group_key(val, names, key_columns) -> tuple:
+    r = pyexec.Row(val if isinstance(val, tuple) else (val,), names)
+    return tuple(r[k] for k in key_columns)
 
 
 def _fits_type(v, t: int) -> bool:
@@ -1033,7 +996,7 @@ def _fits_type(v, t: int) -> bool:
     return isinstance(v, int) and not isinstance(v, bool) and -(1 << 63) <= v < (1 << 63)
 
 
-def _device_merge_csv(held, row_ops, src, input_row, out_types, exc_counter: Counter) -> Optional[List[bytes]]:
+def _device_merge_csv(held, row_ops, names, inputs: Dict[int, Any], out_types, exc_counter: Counter) -> Optional[List[bytes]]:
     """CSV text of every held block result with its resolved exception rows merged in order on the device
     (tplx_gpu_result_merge_resolved + tplx_gpu_result_csv). None when a resolved row does not fit the stage's output schema
     (the host path then merges and formats); exception counts are only taken over on success."""
@@ -1050,14 +1013,10 @@ def _device_merge_csv(held, row_ops, src, input_row, out_types, exc_counter: Cou
             continue
         rows, nos = [], []
         for e in ex[np.argsort(ex["row_no"], kind="stable")]:
-            try:
-                val, _ = pyexec.run_row(row_ops, input_row(lo + int(e["row"])), src.names)
-            except Dropped:
+            r = _run_py(row_ops, inputs[lo + int(e["row"])], names, counts, int(e["op_id"]))
+            if r is None:
                 continue
-            except Exception as err:  # noqa: BLE001 — stays an exception
-                counts[(getattr(err, "tplx_op", int(e["op_id"])), type(err).__name__)] += 1
-                continue
-            vt = val if isinstance(val, tuple) else (val,)
+            vt = r[0] if isinstance(r[0], tuple) else (r[0],)
             if len(vt) != ncols or not all(_fits_type(v, t) for v, t in zip(vt, out_types)):
                 return None
             rows.append(vt)
@@ -1095,9 +1054,9 @@ def _merge_by_rowno(normal_rows: list, excs: np.ndarray, resolved: List[Tuple[in
     return out
 
 
-def _run_stage_python(ctx, src: Source, ops: List[Op], exc_counter: Counter):
+def _run_stage_python(src: Source, ops: List[Op], exc_counter: Counter):
     """Whole stage on the CPython path (UDF outside the GPU op set)."""
-    end = ops[-1] if ops and ops[-1].kind in ("aggregate", "aggregateByKey", "unique") else None
+    end = ops[-1] if ops and ops[-1].kind in _ENDPOINTS else None
     row_ops = ops[:-1] if end else ops
     vals = [c.to_values() for c in src.cols]
     items: List[Tuple[int, Any]] = []
@@ -1106,41 +1065,30 @@ def _run_stage_python(ctx, src: Source, ops: List[Op], exc_counter: Counter):
         items.append((pos, _row_of(src.cols, vals, i)))
     items += list(src.fallback)
     items.sort(key=lambda t: t[0])
-    out = []
-    names = list(src.names)
-    for _, obj in items:
-        try:
-            v, names = pyexec.run_row(row_ops, obj, src.names)
-            out.append(v)
-        except Dropped:
-            pass
-        except Exception as ex:  # noqa: BLE001
-            exc_counter[(getattr(ex, "tplx_op", 0), type(ex).__name__)] += 1
+    out = [r for r in (_run_py(row_ops, obj, src.names, exc_counter, 0) for _, obj in items) if r is not None]  # (value, names)
+    names = out[-1][1] if out else list(src.names)
     if end is None:
-        return out, names
-    if end.kind == "aggregate":
-        combine, init = end.extra
-        agg = end.udf if not isinstance(end.udf, str) else eval(end.udf)
-        value = init
-        for v in out:
-            try:
-                value = agg(value, v)
-            except Exception as ex:  # noqa: BLE001
-                exc_counter[(end.id, type(ex).__name__)] += 1
-        comb = combine if not isinstance(combine, str) else eval(combine)
-        value = comb(init, value)  # thread slot (initial value) combined with the task partial
-        return [value], [None]
+        return [v for v, _ in out], names
     if end.kind == "unique":
-        seen = dict.fromkeys(out)
-        return list(seen), names
+        return list(dict.fromkeys(v for v, _ in out)), names
     combine, init = end.extra
     agg = end.udf if not isinstance(end.udf, str) else eval(end.udf)
     comb = combine if not isinstance(combine, str) else eval(combine)
+    if end.kind == "aggregate":
+        value = init
+        for v, row_names in out:
+            try:
+                value = agg(value, _endpoint_arg(v, row_names))
+            except Exception as ex:  # noqa: BLE001
+                exc_counter[(end.id, type(ex).__name__)] += 1
+        return [comb(init, value)], [None]  # thread slot (initial value) combined with the task partial
     table: Dict[Any, Any] = {}
-    for v in out:
-        r = pyexec.Row(v if isinstance(v, tuple) else (v,), names)
-        key = tuple(r[k] for k in end.columns)
-        table[key] = agg(table.get(key, init), r if len(r) != 1 else r[0])
+    for v, row_names in out:
+        key = _group_key(v, row_names, end.columns)
+        try:
+            table[key] = agg(table.get(key, init), _endpoint_arg(v, row_names))
+        except Exception as ex:  # noqa: BLE001
+            exc_counter[(end.id, type(ex).__name__)] += 1
     rows = []
     for key in sorted(table, key=_key_order):
         v = comb(init, table[key])  # combine at least once per group (LocalBackend.cc:2148-2217)
