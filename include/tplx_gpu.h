@@ -103,7 +103,8 @@ int32_t tplx_gpu_stage_destroy(tplx_stage *stage);
  * sm_90a) and launched instead of the interpreting kernel — same parameters, same tiles / scans / exception records.
  * Controlled by TPLX_JIT (0 off, 1 = stages with blocks of >= TPLX_JIT_MIN_ROWS rows [default], 2 = always); when NVRTC is not
  * installed the interpreting kernels run. This entry point is the diagnostic view of it and needs no device: the generated row
- * function of `kind` (1 = K1 rows, 2 / 3 = K1v with 8 / 4 rows per thread, 4 = K3 aggregate, 5 = K1m mask) as text,
+ * function of `kind` (1 = K1 rows, 2 / 3 = K1v with 8 / 4 rows per thread, 4 = K3 aggregate, 5 = K1m mask, 6 = K1w and 10 = K1r,
+ * the wide-tile fixed-width kernels; any other number is TPLX_E_BADARG) as text,
  * and, with compile != 0, the size of the cubin NVRTC produced for it (0 + the compiler log when it failed / NVRTC is absent). */
 int32_t tplx_gpu_stage_specialise(tplx_stage *stage, int32_t kind, int32_t compile, char *src, uint64_t src_cap, uint64_t *src_len,
                                   uint64_t *cubin_bytes, char *log, uint64_t log_cap);

@@ -358,31 +358,22 @@ def test_fused_idioms_gpu_vs_oracle(gpu, case):
 
 
 @pytest.mark.parametrize("n", [1, 31, 32, 33, 63, 64, 65, 255, 257, 8191, 8192, 8193, 100_003])
-def test_mask_stage_ragged_sizes_and_modes(gpu, n, monkeypatch):
-    """K1m (mask.cuh): bitmaps + survivor list for every tail shape; staged (TMA ring) == unstaged (global loads) == old
-    look-back prefilter (TPLX_NO_MASK=1) == oracle; MR = 1 and 2 rows per lane."""
+def test_mask_stage_ragged_sizes_and_modes(gpu, n):
+    """K1m (mask.cuh): bitmaps + survivor list for every tail shape == oracle."""
     import idiom_udfs as U
     cols, _ = U.make_columns(n, n)
     prog = _idiom_prog(U.number_before_marker, True)
     ora = pyoracle.run_program(prog, cols, n, 11)
-    for env in ({}, {"TPLX_MASK_STAGE": "1"}, {"TPLX_MASK_STAGE": "1", "TPLX_MASK_MR": "2"}, {"TPLX_MASK_MR": "2"}, {"TPLX_NO_MASK": "1"}):
-        for k in ("TPLX_MASK_STAGE", "TPLX_MASK_MR", "TPLX_NO_MASK"):
-            monkeypatch.delenv(k, raising=False)
-        for k, v in env.items():
-            monkeypatch.setenv(k, v)
-        res = backend.Stage(prog).run_host(0, cols, n, 11)
-        assert_result_equals_oracle(res, ora, f"n={n} env={env}")
+    res = backend.Stage(prog).run_host(0, cols, n, 11)
+    assert_result_equals_oracle(res, ora, f"n={n}")
 
 
-def test_mask_stage_oversized_rows_fall_back_to_global(gpu, monkeypatch):
-    monkeypatch.setenv("TPLX_MASK_STAGE", "1")
-    _oversized_rows_check()
-    monkeypatch.setenv("TPLX_MASK_STAGE", "0")
+def test_mask_stage_long_strings_between_short_ones(gpu):
     _oversized_rows_check()
 
 
 def _oversized_rows_check():
-    """Tiles whose string bytes exceed the ring slot keep their global pointers: rare very long strings between short ones."""
+    """Rare very long strings (up to 12 KB) between short ones, through the prefilter and the dense launch."""
     rng = np.random.default_rng(5)
     n = 30_000
     base = ["3 bds , 2 ba", "1 bd", "x", "", "12 bds , 1 ba , 700 sqft"]
@@ -456,8 +447,8 @@ def test_vector_kernel_equals_scalar_kernel_and_oracle(gpu, n, monkeypatch):
 @pytest.mark.parametrize("n", [1, 33, 50_001])
 def test_string_scan_closed_form_equals_vm_and_oracle(gpu, name, n, monkeypatch):
     """K1f: the prefilter evaluated from the string-scan hint (closed form, no interpretation) == the same stage through the VM
-    (TPLX_NO_SCAN=1) == the old look-back prefilter (TPLX_NO_MASK=1) == oracle (which only ever runs the program): kept rows,
-    exception rows (ValueError of int() attributed to the withColumn operator), row numbers."""
+    (TPLX_NO_SCAN=1) == oracle (which only ever runs the program): kept rows, exception rows (ValueError of int() attributed to the
+    withColumn operator), row numbers."""
     import scan_udfs as U
     head = {h[0]: h[1] for h in U.HINTED}[name]
     sc = frontend.StageCompiler(U.TYPES, U.NAMES)
@@ -467,9 +458,8 @@ def test_string_scan_closed_form_equals_vm_and_oracle(gpu, name, n, monkeypatch)
     assert prog.prefilter is not None and ir.scan_terms(prog.prefilter.fused) is not None
     cols = U.make_columns(n, n)
     ora = pyoracle.run_program(prog, cols, n, 4)
-    for env in ({}, {"TPLX_NO_SCAN": "1"}, {"TPLX_MASK_STAGE": "1"}, {"TPLX_NO_SCAN": "1", "TPLX_MASK_STAGE": "1"}, {"TPLX_NO_MASK": "1"}):
-        for k in ("TPLX_NO_SCAN", "TPLX_MASK_STAGE", "TPLX_NO_MASK"):
-            monkeypatch.delenv(k, raising=False)
+    for env in ({}, {"TPLX_NO_SCAN": "1"}):
+        monkeypatch.delenv("TPLX_NO_SCAN", raising=False)
         for k, v in env.items():
             monkeypatch.setenv(k, v)
         res = backend.Stage(prog).run_host(0, cols, n, 4)

@@ -7,6 +7,7 @@ workload and random programs. GPU part: with TPLX_JIT=2 (every stage specialised
 the oracle and to the interpreting kernels (TPLX_JIT=0), and the result reports that specialised kernels really ran."""
 import hashlib
 import os
+import re
 
 import numpy as np
 import pytest
@@ -16,7 +17,7 @@ from oracle import pyoracle
 from fuzz_udfs import COLS, TYPES, Gen, apply_ops, make_columns
 from helpers import assert_result_equals_oracle
 
-K_ROWS, K_VEC4, K_VEC2, K_AGG, K_MASK = 1, 2, 3, 4, 5
+K_ROWS, K_VEC4, K_VEC2, K_AGG, K_MASK, K_WIDE4, K_RE2 = 1, 2, 3, 4, 5, 6, 10
 
 
 class jit_mode:
@@ -49,6 +50,17 @@ def test_c1_row_function_text_and_cubin():
     assert nb > 0, f"NVRTC produced no cubin: {log}"
     src1, nb1, log1 = st.specialise(K_ROWS)
     assert "jit_run(" in src1 and nb1 > 0, log1
+    st.close()
+
+
+def test_wide_tile_kinds_compile_and_other_numbers_are_rejected():
+    st = backend.Stage(W.c1_program())
+    for kind in (K_WIDE4, K_RE2):
+        src, nb, log = st.specialise(kind)
+        assert "jit_row_fixed" in src and nb > 0, log
+    for kind in (0, 7, 8, 9, 11, 12):
+        with pytest.raises(backend.GpuBackendError):
+            st.specialise(kind)
     st.close()
 
 
@@ -283,38 +295,48 @@ def test_tiered_execution_background_compile(gpu):
                 os.environ[k] = v
 
 
+# Program shapes and the specialised fixed-width kernel each one selects (run_rows_vec): at most 16 instructions -> K1r; else K1w
+# when the live-out slots of four 2048-row sub-batches fit 74 KB of shared memory (one slot); else K1v with J = 4 when they fit 56 KB
+# (two slots), else with J = 2 within 100 KB (three to eleven slots). name: (more than 16 instructions, final map, kind)
+WIDE_SHAPES = {
+    "re2": (False, None, K_RE2),
+    "re2_2out": (False, lambda x: (x, x * 2 + 1), K_RE2),
+    "wide4": (True, None, K_WIDE4),
+    "vec4": (True, lambda x: (x, x * 2 + 1), K_VEC4),
+    "vec2": (True, lambda x: (x, x * 2 + 1, x - 5), K_VEC2),
+    "vec2_11out": (True, lambda x: (x, x + 1, x + 2, x + 3, x + 4, x + 5, x + 6, x + 7, x + 8, x + 9, x + 10), K_VEC2),
+}
+
+
 @pytest.mark.gpu
 @pytest.mark.parametrize("n", [1, 8191, 8192, 8193, 16385, 100_003, 3_000_001])
-@pytest.mark.parametrize("kernel", ["re2", "re4", "re8", "wide4", "wide2", "k1v"])
-def test_wide_tile_kernels_with_exceptions(gpu, n, kernel):
-    """The specialised fixed-width kernels with tiles wider than K1v's 2048 rows vs the oracle — K1r (nothing staged, the tile is
-    evaluated again from L2 once its offset is known; 2 / 4 / 8 sub-batches of 2048 rows per ticket, two tiles in flight per CTA) and K1w (live-out slots of 4 / 2
-    sub-batches staged in shared memory) — on ragged tiles, with ZeroDivisionError rows, a filter, one and two output columns."""
+@pytest.mark.parametrize("shape", list(WIDE_SHAPES))
+def test_wide_tile_kernels_with_exceptions(gpu, n, shape, monkeypatch, capfd):
+    """The specialised fixed-width kernels vs the oracle, each selected by the shape of its program — K1r (nothing staged, the tile is
+    evaluated again from L2 once its offset is known; 2 sub-batches of 2048 rows per ticket, two tiles in flight per CTA), K1w (live-out
+    slots of 4 sub-batches staged in shared memory), K1v with J = 4 and J = 2 — on ragged tiles, with ZeroDivisionError rows and a filter.
+    The trace names the kind that was loaded."""
+    long, final_map, kind = WIDE_SHAPES[shape]
     rng = np.random.default_rng(n)
     a = rng.integers(-10_000, 10_000, n)
     cols = [backend.Column(ir.T_I64, a)]
-    env = {"re2": ("2", "0"), "re4": ("4", "0"), "re8": ("8", "0"), "wide4": ("0", "4"), "wide2": ("0", "2"), "k1v": ("0", "0")}[kernel]
-    old = {k: os.environ.get(k) for k in ("TPLX_JIT_RE", "TPLX_JIT_WIDE")}
-    os.environ["TPLX_JIT_RE"], os.environ["TPLX_JIT_WIDE"] = env
-    try:
-        for two in (False, True):
-            sc = frontend.StageCompiler([ir.T_I64], ["a"])
-            sc.add_map(lambda x: x // (x % 7), 100001)       # x % 7 == 0 raises
-            sc.add_filter(lambda x: x % 3 != 1, 100002)
-            if two:
-                sc.add_map(lambda x: (x, x * 2 + 1), 100003)
-            prog = sc.finish_memory(prefilter=False)
-            ora = pyoracle.run_program(prog, cols, n, first_row_no=5)
-            with jit_mode(2):
-                st = backend.Stage(prog)
-                res = st.run_host(0, cols, n, first_row_no=5)
-                assert_result_equals_oracle(res, ora, f"n={n} kernel={kernel} two={two}")
-                assert int(res.info.specialised_launches) > 0
-                res.free()
-                st.close()
-    finally:
-        for k, v in old.items():
-            if v is None:
-                os.environ.pop(k, None)
-            else:
-                os.environ[k] = v
+    sc = frontend.StageCompiler([ir.T_I64], ["a"])
+    sc.add_map(lambda x: x // (x % 7), 100001)       # x % 7 == 0 raises
+    sc.add_filter(lambda x: x % 3 != 1, 100002)
+    if long:
+        sc.add_map(lambda x: ((x * 3 + 1) ^ (x >> 2)) + ((x * 5 - 7) & 1023) - (x | 96) + (x << 1), 100003)
+    if final_map is not None:
+        sc.add_map(final_map, 100004)
+    prog = sc.finish_memory(prefilter=False)
+    assert (len(prog.instrs) > 16) == long
+    ora = pyoracle.run_program(prog, cols, n, first_row_no=5)
+    monkeypatch.setenv("TPLX_TRACE", "1")
+    capfd.readouterr()
+    with jit_mode(2):
+        st = backend.Stage(prog)
+        res = st.run_host(0, cols, n, first_row_no=5)
+        assert_result_equals_oracle(res, ora, f"n={n} shape={shape}")
+        assert int(res.info.specialised_launches) > 0
+        res.free()
+        st.close()
+    assert re.findall(r"specialiser: kind (\d+) loaded", capfd.readouterr().err) == [str(kind)]

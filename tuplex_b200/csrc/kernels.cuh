@@ -42,11 +42,12 @@ struct AccP {
 struct KParams {
     uint64_t n_rows;
     int64_t first_row_no;
-    uint32_t n_instr, pad_split, n_slots, n_in, n_out, n_str_out, n_accs, R, n_tiles, scratch_per_thread;
+    uint32_t n_instr;
+    uint32_t inplace;         // 1: one row per thread and no staging area — outputs are read from the register file (slot s of local row lr = regs[s][lr])
+    uint32_t n_slots, n_in, n_out, n_str_out, n_accs, R, n_tiles, scratch_per_thread;
     uint32_t K;            // scan vector width = 2 + n_str_out
     uint32_t smem_regs_off, smem_stage_off, smem_misc_off, smem_cols_off;
     uint32_t smem_stash_off;  // per string output column: NT/32 warp totals of the byte scan
-    uint32_t inplace;         // 1: one row per thread and no staging area — outputs are read from the register file (slot s of local row lr = regs[s][lr])
     uint64_t cap_rows, cap_exc;
     const DInstr *prog;    // pre-decoded program (device format)
     const uint8_t *cpool;
@@ -324,11 +325,11 @@ __device__ __forceinline__ void rows_tile_finish(const KParams &P, const TileSme
 // ---- stage specialiser (jit.inl) ----------------------------------------------------------------------------------------------
 // When this header is compiled at run time by NVRTC (TPLX_JIT), "jit_row.cuh" is the op program of ONE stage printed as a
 // straight-line function (jit_run / jit_row_fixed) and exactly one kernel of the library is compiled around it, as
-// `tplx_jit_kernel`: TPLX_JIT_KIND 1 = K1 rows, 2 / 3 = K1v (J = 4 / 2), 4 = K3 aggregate, 5 = K1m mask (K4, the hash aggregate, is table-bound and stays interpreted).
+// `tplx_jit_kernel`: TPLX_JIT_KIND 1 = K1 rows, 2 / 3 = K1v (J = 4 / 2), 4 = K3 aggregate, 5 = K1m mask, 6 = K1w, 10 = K1r
+// (K4, the hash aggregate, is table-bound and stays interpreted). TPLX_JIT_MIN_CTAS is the kernel's second __launch_bounds__ argument.
 // The register file of a specialised kernel is COMPACT: it holds the live-out slots only (outputs, accumulator inputs), in the
 // order the host's jit::liveout() numbered them; KParams carries those compact slot numbers.
 #ifdef TPLX_JIT
-__device__ __forceinline__ void jit_touch(const void *p) { asm volatile("prefetch.global.L1 [%0];" ::"l"(p)); }
 #include "jit_row.cuh"
 #define TPLX_VM_RUN(prog, n_instr, regs, cols, row, w, cpool, t) jit_run(regs, cols, row, w, cpool, t)
 #else
@@ -342,7 +343,7 @@ __device__ __forceinline__ void jit_touch(const void *p) { asm volatile("prefetc
 // misc: keep_bits[W] exc_bits[W] keep_pre[W+1] exc_pre[W+1] exc_stage[T] scan scratch
 #if !defined(TPLX_JIT) || TPLX_JIT_KIND == 1
 #ifdef TPLX_JIT
-extern "C" __global__ void __launch_bounds__(NT, TPLX_JIT_MINB) tplx_jit_kernel(const __grid_constant__ KParams P) {
+extern "C" __global__ void __launch_bounds__(NT, TPLX_JIT_MIN_CTAS) tplx_jit_kernel(const __grid_constant__ KParams P) {
 #else
 __global__ void __launch_bounds__(NT) stage_rows_kernel(const __grid_constant__ KParams P) {  // parameters in the constant bank
 #endif
@@ -426,9 +427,6 @@ __global__ void __launch_bounds__(NT) stage_rows_kernel(const __grid_constant__ 
             const uint64_t row = P.rowlist ? (valid ? P.rowlist[w] : 0) : w;
             t.alive = valid;
             t.exc_code = 0;
-#ifdef TPLX_JIT
-            if (P.rowlist && valid && !P.pad_split) jit_prefetch(s_cols, row, w);  // pad_split = 1: switched off (TPLX_JIT_PREFETCH=0)
-#endif
             TPLX_VM_RUN(s_prog, P.n_instr, s_regs, s_cols, row, w, P.cpool, t);
             const bool exc = t.exc_code != 0;
             const uint32_t kb = __ballot_sync(0xFFFFFFFFu, t.alive);
@@ -455,7 +453,7 @@ __global__ void __launch_bounds__(NT) stage_rows_kernel(const __grid_constant__ 
 // =============================================================================================
 #if !defined(TPLX_JIT) || TPLX_JIT_KIND == 4
 #ifdef TPLX_JIT
-extern "C" __global__ void __launch_bounds__(NT, TPLX_JIT_MINB) tplx_jit_kernel(const KParams *__restrict__ Pg) {
+extern "C" __global__ void __launch_bounds__(NT, TPLX_JIT_MIN_CTAS) tplx_jit_kernel(const KParams *__restrict__ Pg) {
 #else
 __global__ void __launch_bounds__(NT) stage_agg_kernel(const KParams *__restrict__ Pg) {
 #endif

@@ -7,37 +7,25 @@
 // here the leading operators up to the selective filter run over every row and only the survivors reach the dense
 // launch (kernels.cuh) that evaluates the whole stage and writes rows.
 //
-// Execution model: every WARP is autonomous. It owns warp-tiles of 32*MR consecutive rows (tile t -> warp
-// t mod #warps), a private 2-deep shared-memory ring, and one mbarrier per ring slot. For tile k+1 the lanes
-// 0..n_staged-1 each bring one string column's byte range [offsets[r0], offsets[r1]) and its offsets into the ring
-// with cp.async.bulk (TMA bulk copy, SASS UBLKCP; completion counted on the mbarrier), while the warp evaluates
-// tile k out of shared memory: the VM's string primitives then read shared memory (~30 cycles) instead of
-// L2/HBM. A tile whose byte range exceeds the ring slot simply keeps its global pointers (always correct).
+// Execution model: every WARP is autonomous. It owns warp-tiles of 32 consecutive rows (tile t -> warp t mod #warps),
+// one row per lane, and reads the input columns from global memory: coalesced offsets, string bytes through L1. The kernel
+// is issue-bound rather than latency-bound, so it spends no instructions on staging tiles in shared memory. The one
+// block-wide barrier publishes the program and the column table.
 // Results: keep_words[t] / exc_words[t] = warp ballots (bit l = row 32 t + l); exc_codes[row] for exception rows only.
 // mask_count / mask_scan / mask_expand turn the bitmaps into the ascending survivor list and the exception records.
 #pragma once
 #include <stdint.h>
 #include "kernels.cuh"
-#include "fused.cuh"
 
 namespace tplx {
 
-constexpr uint32_t MASK_MAX_STAGED = 4;
 constexpr uint32_t MASK_WARPS = NT / 32;
-constexpr uint32_t MASK_RING = 2;
 
 struct MaskParams {
     uint64_t n_rows;
-    uint32_t n_instr, n_in, n_slots, n_tiles;  // n_tiles = warp-tiles of 32*MR rows
-    uint32_t n_staged, MR;
+    uint32_t n_instr, n_in, n_slots, n_tiles;  // n_tiles = warp-tiles of 32 rows
     uint32_t scratch_per_thread;
-    uint32_t smem_regs_off, smem_wcols_off, smem_bar_off, smem_info_off, smem_ring_off;
-    uint32_t slot_bytes;                   // one ring slot of one warp (all staged columns)
-    uint32_t off_bytes;                    // bytes of the staged offsets of one column: (32*MR + 1) * 4 rounded up to 16
-    uint32_t st_col[MASK_MAX_STAGED];      // input column of each staged column
-    uint32_t st_cap[MASK_MAX_STAGED];      // byte capacity (multiple of 16) of its string bytes in a ring slot
-    uint32_t st_boff[MASK_MAX_STAGED];     // where its bytes live inside a ring slot
-    uint32_t st_ooff[MASK_MAX_STAGED];     // where its offsets live inside a ring slot
+    uint32_t smem_regs_off, smem_cols_off;
     const DInstr *prog;
     const uint8_t *cpool;
     uint32_t n_terms;                      // > 0: closed-form evaluation of the stage (string-scan hint), the program is not interpreted
@@ -47,10 +35,6 @@ struct MaskParams {
     uint8_t *scratch;
     ColIn in[TPLX_MAX_COLS];
 };
-
-__device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t *bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
 
 // ---- K1f: closed-form evaluation of a string-scan hint (include/tplx_ir.h tplx_scan_term) ---------------------------------------
 // The same string primitives as the VM's ops (strops.cuh), called directly: no instruction fetch / decode / register file.
@@ -80,13 +64,11 @@ __device__ __forceinline__ bool cmp_f64(uint32_t cmp, double x, double y) {  // 
         default: return x >= y;
     }
 }
-template <bool GLOBAL_ONLY>
 __device__ __forceinline__ StrV scan_col(const ColIn &ci, uint64_t row) {
     StrV s;
-    if (GLOBAL_ONLY) {  // nothing is staged: the column lives in global memory, so the string primitives can use LDG instead of generic LD
-        __builtin_assume(__isGlobal(ci.data));
-        __builtin_assume(__isGlobal(ci.offsets));
-    }
+    // the column lives in global memory, so the string primitives can use LDG instead of generic LD
+    __builtin_assume(__isGlobal(ci.data));
+    __builtin_assume(__isGlobal(ci.offsets));
     const uint32_t o0 = ci.offsets[row], o1 = ci.offsets[row + 1];
     s.p = reinterpret_cast<const uint8_t *>(ci.data) + o0;
     s.len = o1 - o0;
@@ -101,7 +83,6 @@ __device__ __forceinline__ StrV scan_const(const uint8_t *cpool, uint64_t enc) {
     return v;
 }
 // evaluates the terms in order for one row; a row raises only in a term it reaches (PipelineBuilder.cc:949)
-template <bool GLOBAL_ONLY>
 __device__ __forceinline__ void scan_eval(const MaskParams &P, const ColIn *__restrict__ cols, uint64_t row, VMThread &t) {
     for (uint32_t k = 0; k < P.n_terms; ++k) {
         if (!__any_sync(0xFFFFFFFFu, t.alive)) break;
@@ -109,14 +90,14 @@ __device__ __forceinline__ void scan_eval(const MaskParams &P, const ColIn *__re
         if (!t.alive) continue;
         const ColIn &ci = cols[T.col];
         if (T.kind == TPLX_SK_CONTAINS) {
-            StrV s = scan_col<GLOBAL_ONLY>(ci, row);
+            StrV s = scan_col(ci, row);
             const StrV n = scan_const(P.cpool, T.needle);
             const uint32_t cf = T.flags & TPLX_SCF_CASE_MASK;
             s.flags = cf;
             const int64_t r = cf == TPLX_SF_LOWER ? scan_find<TPLX_SF_LOWER>(s, n) : (cf == TPLX_SF_UPPER ? scan_find<TPLX_SF_UPPER>(s, n) : scan_find<TPLX_SF_NONE>(s, n));
             t.alive = (r >= 0) != ((T.flags & TPLX_SCF_NEGATE) != 0);
         } else if (T.kind == TPLX_SK_FIELD_INT) {
-            const StrV s = scan_col<GLOBAL_ONLY>(ci, row);
+            const StrV s = scan_col(ci, row);
             const int64_t i = scan_find<TPLX_SF_NONE>(s, scan_const(P.cpool, T.needle));
             StrV head = s;
             head.len = i < 0 ? s.len : (uint32_t)i;                                   // s[:stop]
@@ -144,37 +125,29 @@ __device__ __forceinline__ void scan_eval(const MaskParams &P, const ColIn *__re
 
 // The parameter block travels by value in the kernel's constant bank (__grid_constant__): every P.field below is a constant-bank
 // operand instead of a global load through a pointer (terms, column table, offsets — read in the per-row loops).
-// MINB: resident CTAs per SM the register allocation must allow (4 = 64 registers, 5 = 48, 6 = 40).
+// __launch_bounds__(NT, 4): 4 resident CTAs per SM, 64 registers per thread.
 #if !defined(TPLX_JIT) || TPLX_JIT_KIND == 5
 #ifdef TPLX_JIT
 // specialised K1m (stage specialiser, jit.inl): the prefilter program as straight-line code, no register file at all (the bitmaps carry the result)
-extern "C" __global__ void __launch_bounds__(NT, TPLX_JIT_MINB) tplx_jit_kernel(const __grid_constant__ MaskParams P) {
+extern "C" __global__ void __launch_bounds__(NT, TPLX_JIT_MIN_CTAS) tplx_jit_kernel(const __grid_constant__ MaskParams P) {
     constexpr bool SCAN = false;
 #else
-template <bool SCAN, int MINB = 4>
-__global__ void __launch_bounds__(NT, MINB) stage_mask_kernel(const __grid_constant__ MaskParams P) {
+template <bool SCAN>
+__global__ void __launch_bounds__(NT, 4) stage_mask_kernel(const __grid_constant__ MaskParams P) {
 #endif
     extern __shared__ __align__(16) uint8_t smem[];
     const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const uint32_t MR = P.MR, TR = 32 * MR, ns = P.n_staged;
 
     DInstr *s_prog = reinterpret_cast<DInstr *>(smem);
     uint8_t *s_regs = smem + P.smem_regs_off + tid * 8;
-    ColIn *s_wcols = reinterpret_cast<ColIn *>(smem + P.smem_wcols_off) + warp * P.n_in;          // this warp's column table
-    uint64_t *bars = reinterpret_cast<uint64_t *>(smem + P.smem_bar_off) + warp * MASK_RING;
-    uint32_t *info = reinterpret_cast<uint32_t *>(smem + P.smem_info_off) + warp * MASK_RING * 2 * MASK_MAX_STAGED;
-    uint8_t *ring = smem + P.smem_ring_off + (size_t)warp * MASK_RING * P.slot_bytes;
+    ColIn *s_cols = reinterpret_cast<ColIn *>(smem + P.smem_cols_off);
 
     if (!SCAN)
         for (uint32_t i = tid; i < P.n_instr * (sizeof(DInstr) / 16); i += NT)
             reinterpret_cast<uint4 *>(s_prog)[i] = reinterpret_cast<const uint4 *>(P.prog)[i];
-    for (uint32_t i = lane; i < P.n_in * (sizeof(ColIn) / 8); i += 32)
-        reinterpret_cast<uint64_t *>(s_wcols)[i] = reinterpret_cast<const uint64_t *>(P.in)[i];
-    if (lane == 0 && ns) {
-        for (uint32_t s = 0; s < MASK_RING; ++s) mbar_init(&bars[s], ns);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncthreads();  // the only block-wide barrier: program + barriers ready
+    for (uint32_t i = tid; i < P.n_in * (sizeof(ColIn) / 8); i += NT)
+        reinterpret_cast<uint64_t *>(s_cols)[i] = reinterpret_cast<const uint64_t *>(P.in)[i];
+    __syncthreads();  // the only block-wide barrier: program + column table ready
 
     VMThread t;
     t.scr_cap = P.scratch_per_thread;
@@ -182,77 +155,22 @@ __global__ void __launch_bounds__(NT, MINB) stage_mask_kernel(const __grid_const
 
     const uint32_t gw = blockIdx.x * MASK_WARPS + warp, GW = gridDim.x * MASK_WARPS;
     const uint32_t my_tiles = P.n_tiles > gw ? (P.n_tiles - gw + GW - 1) / GW : 0;
-
-    // lane k < ns stages column st_col[k] of a tile into ring slot `slot`
-    const bool stager = lane < ns;
-    const ColIn my_col = stager ? P.in[P.st_col[lane]] : ColIn{};
-    const bool offs_aligned = stager && ((reinterpret_cast<uintptr_t>(my_col.offsets) & 15) == 0);
-    auto issue = [&](uint32_t q, uint32_t o0, uint32_t o1) {
-        const uint32_t slot = q % MASK_RING;
-        const uint64_t r0 = (uint64_t)(gw + (uint64_t)q * GW) * TR;
-        const uint32_t a0 = o0 & ~15u;
-        const uint32_t nb = ((o1 + 15u) & ~15u) - a0;
-        const bool sb = nb != 0 && nb <= P.st_cap[lane];
-        const bool so = offs_aligned && r0 + P.off_bytes / 4 <= P.n_rows + 1;
-        uint32_t *inf = info + slot * 2 * MASK_MAX_STAGED;
-        inf[lane] = sb ? a0 : 0xFFFFFFFFu;
-        inf[MASK_MAX_STAGED + lane] = so;
-        mbar_arrive_expect_tx(&bars[slot], (sb ? nb : 0u) + (so ? P.off_bytes : 0u));
-        uint8_t *dst = ring + (size_t)slot * P.slot_bytes;
-        if (sb) bulk_g2s(dst + P.st_boff[lane], reinterpret_cast<const uint8_t *>(my_col.data) + a0, nb, &bars[slot]);
-        if (so) bulk_g2s(dst + P.st_ooff[lane], my_col.offsets + r0, P.off_bytes, &bars[slot]);
-    };
-    auto tile_range = [&](uint32_t q, uint32_t &o0, uint32_t &o1) {  // byte range of tile q of this warp in my column
-        const uint64_t r0 = (uint64_t)(gw + (uint64_t)q * GW) * TR;
-        const uint64_t r1 = r0 + TR < P.n_rows ? r0 + TR : P.n_rows;
-        o0 = my_col.offsets[r0];
-        o1 = my_col.offsets[r1];
-    };
-    uint32_t no0 = 0, no1 = 0;  // range of the next tile to issue (loaded one iteration ahead)
-    if (stager && my_tiles) {
-        tile_range(0, no0, no1);
-        issue(0, no0, no1);
-        if (my_tiles > 1) tile_range(1, no0, no1);
-    }
-
     for (uint32_t q = 0; q < my_tiles; ++q) {
-        const uint32_t slot = q % MASK_RING;
         const uint64_t tile = gw + (uint64_t)q * GW;
-        const uint64_t r0 = tile * TR;
-        if (ns) {
-            if (stager && q + 1 < my_tiles) {
-                issue(q + 1, no0, no1);  // slot (q+1)%2 was released by the __syncwarp that ended iteration q-1
-                if (q + 2 < my_tiles) tile_range(q + 2, no0, no1);
-            }
-            mbar_wait(&bars[slot], (q / MASK_RING) & 1);
-            if (stager) {
-                const uint32_t *inf = info + slot * 2 * MASK_MAX_STAGED;
-                const uint32_t a0 = inf[lane];
-                const uint8_t *base = ring + (size_t)slot * P.slot_bytes;
-                ColIn &wc = s_wcols[P.st_col[lane]];
-                // views are formed as data + offsets[row]: rebase both so that the sums land inside the ring slot
-                wc.data = a0 != 0xFFFFFFFFu ? static_cast<const void *>(base + P.st_boff[lane] - a0) : my_col.data;
-                wc.offsets = inf[MASK_MAX_STAGED + lane] ? reinterpret_cast<const uint32_t *>(base + P.st_ooff[lane]) - r0 : my_col.offsets;
-            }
-            __syncwarp();
+        const uint64_t row = tile * 32 + lane;
+        t.alive = row < P.n_rows;
+        t.exc_code = 0;
+        t.scr_used = 0;
+        if (SCAN) scan_eval(P, s_cols, row, t);
+        else TPLX_VM_RUN(s_prog, P.n_instr, s_regs, s_cols, row, row, P.cpool, t);
+        const bool exc = t.exc_code != 0;
+        const uint32_t kb = __ballot_sync(0xFFFFFFFFu, t.alive);
+        const uint32_t eb = __ballot_sync(0xFFFFFFFFu, exc);
+        if (lane == 0) {
+            P.keep_words[tile] = kb;
+            P.exc_words[tile] = eb;
         }
-        for (uint32_t s = 0; s < MR; ++s) {
-            const uint64_t row = r0 + (uint64_t)s * 32 + lane;
-            t.alive = row < P.n_rows;
-            t.exc_code = 0;
-            t.scr_used = 0;
-            if (SCAN) { if (ns) scan_eval<false>(P, s_wcols, row, t); else scan_eval<true>(P, s_wcols, row, t); }
-            else TPLX_VM_RUN(s_prog, P.n_instr, s_regs, s_wcols, row, row, P.cpool, t);
-            const bool exc = t.exc_code != 0;
-            const uint32_t kb = __ballot_sync(0xFFFFFFFFu, t.alive);
-            const uint32_t eb = __ballot_sync(0xFFFFFFFFu, exc);
-            if (lane == 0) {
-                P.keep_words[tile * MR + s] = kb;
-                P.exc_words[tile * MR + s] = eb;
-            }
-            if (exc) P.exc_codes[row] = t.exc_code | (t.exc_op << 16);
-        }
-        __syncwarp();  // every lane is done with this ring slot
+        if (exc) P.exc_codes[row] = t.exc_code | (t.exc_op << 16);
     }
 }
 #endif  // K1m

@@ -116,13 +116,10 @@ extern "C" int32_t tplx_gpu_init(const int32_t *devices, int32_t n) {
         CU(cudaFuncSetAttribute(stage_hash_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, d->smem_optin));
         CU(cudaFuncSetAttribute(stage_hash_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, d->smem_optin));
         CU(cudaFuncSetAttribute(stage_mask_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, d->smem_optin));
-        CU(cudaFuncSetAttribute(stage_mask_kernel<true, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, d->smem_optin));
-        CU(cudaFuncSetAttribute(stage_mask_kernel<true, 5>, cudaFuncAttributeMaxDynamicSharedMemorySize, d->smem_optin));
-        CU(cudaFuncSetAttribute(stage_mask_kernel<true, 6>, cudaFuncAttributeMaxDynamicSharedMemorySize, d->smem_optin));
-        // extra execution lanes on the same GPU (chain d -> alt -> alt ...): TPLX_LANES lanes in all. Two lanes let the
-        // latency-bound dense launch of one block overlap the prefilter of the next; the default is 2.
-        int lanes = 2;
-        if (const char *e = getenv("TPLX_LANES")) lanes = std::max(1, std::min(8, atoi(e)));
+        CU(cudaFuncSetAttribute(stage_mask_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, d->smem_optin));
+        // extra execution lanes on the same GPU (chain d -> alt -> alt ...): two lanes in all let the latency-bound dense
+        // launch of one block overlap the prefilter of the next
+        constexpr int lanes = 2;
         Device *tail = d;
         for (int l = 1; l < lanes; ++l) {
             Device *a = new Device();
@@ -704,17 +701,15 @@ static std::shared_ptr<jit::Binary> jit_binary(tplx_stage *s, int kind, int minb
     else bin->worker = std::thread(jit_compile_job, bin, std::move(src), kind, minb, s->instrs.size());
     return bin;
 }
-// resident CTAs per SM the specialised kernel's register allocation must allow (TPLX_JIT_MINB* override them)
+// resident CTAs per SM the specialised kernel's register allocation must allow
 static int jit_minb(const tplx_stage *s, int kind) {
-    auto env = [](const char *n, int dflt) { const char *e = getenv(n); return e && atoi(e) > 0 ? atoi(e) : dflt; };
     switch (kind) {
-        case jit::K_VEC4: return env("TPLX_JIT_MINB_VEC", 8);
-        case jit::K_WIDE4: return env("TPLX_JIT_MINB_WIDE", 3);
-        case jit::K_WIDE2: return env("TPLX_JIT_MINB_WIDE", 4);
-        case jit::K_RE4: case jit::K_RE8: case jit::K_RE2: case jit::K_RE1: return env("TPLX_JIT_MINB_RE", 6);
-        case jit::K_VEC2: return env("TPLX_JIT_MINB_VEC", 3);
-        case jit::K_MASK: return env("TPLX_JIT_MINB_MASK", 4);
-        default: return env("TPLX_JIT_MINB", 3);
+        case jit::K_VEC4: return 8;
+        case jit::K_WIDE4: return 3;
+        case jit::K_RE2: return 6;
+        case jit::K_VEC2: return 3;
+        case jit::K_MASK: return 4;
+        default: return 3;
     }
 }
 static bool jit_wanted(tplx_stage *s, uint64_t block_rows) {
@@ -824,8 +819,8 @@ extern "C" int32_t tplx_gpu_stage_vec_plan(const tplx_stage *s, tplx_vec_uop *ou
 
 extern "C" int32_t tplx_gpu_stage_specialise(tplx_stage *s, int32_t kind, int32_t compile, char *src, uint64_t src_cap, uint64_t *src_len,
                                              uint64_t *cubin_bytes, char *log, uint64_t log_cap) {
-    if (!s || kind < jit::K_ROWS || kind > jit::K_RE1) return fail(TPLX_E_BADARG, "stage_specialise: bad arguments");
-    if ((kind == jit::K_VEC4 || kind == jit::K_VEC2 || kind >= jit::K_WIDE4) && !s->vec_ok) return fail(TPLX_E_UNSUPPORTED, "stage_specialise: not a fixed-width MEMORY stage");
+    if (!s || !jit::is_kind(kind)) return fail(TPLX_E_BADARG, "stage_specialise: bad arguments");
+    if (jit::is_fixed_width(kind) && !s->vec_ok) return fail(TPLX_E_UNSUPPORTED, "stage_specialise: not a fixed-width MEMORY stage");
     std::string text;
     size_t nb = 0;
     std::string lg;
@@ -1061,6 +1056,18 @@ static Layout make_layout(const tplx_stage *s, uint32_t R, bool rows_ep, bool in
         off += (size_t)(NT / 32) * std::max<size_t>(s->accs.size(), 1) * 8;
     }
     L.total = (uint32_t)align_up(off, 16);
+    return L;
+}
+// shared-memory layout of the fixed-width kernels (vecvm.cuh) with T-row tiles: program (16 bytes in a specialised kernel) | cols |
+// register file (output columns are staged in place: a slot is indexed by the local row) | misc: 32 group counts per 2048-row
+// sub-batch, K1v's exception codes (exc_codes: one word per row of the tile), look-back scratch, ticket
+static Layout vec_layout(const tplx_stage *s, size_t prog_bytes, uint32_t T, size_t regs_bytes, bool exc_codes) {
+    Layout L;
+    L.cols_off = (uint32_t)align_up(prog_bytes, 16);
+    L.regs_off = L.stage_off = (uint32_t)align_up(L.cols_off + std::max<size_t>(s->in_types.size(), 1) * sizeof(ColIn), 16);
+    L.misc_off = (uint32_t)align_up(L.regs_off + regs_bytes, 16);
+    const size_t misc = (size_t)std::max<uint32_t>(T / 2048, 1) * 32 * 4 + (exc_codes ? (size_t)T * 4 : 0) + (size_t)(4 * (NT / 32)) * 8 + 16;
+    L.total = (uint32_t)align_up(L.misc_off + misc, 16);
     return L;
 }
 
@@ -1367,96 +1374,53 @@ static int32_t run_rows_vec(tplx_stage *s, StageDev *sd, const tplx_block *b, in
     const size_t n_uops = s->vplan.ins.size();
     // J = 4 (2048-row tiles, 8 rows per thread per dispatch) when the register file leaves room for >= 3 CTAs per SM, else J = 2
     int Jsel = 0;
-    uint32_t smem = 0, T = 0, cols_off = 0, regs_off = 0, misc_off = 0;
+    uint32_t T = 0;
+    Layout L;
     for (int J : {4, 2}) {
         T = 2u * J * NT;
-        size_t off = align_up(std::max<size_t>(n_uops, 1) * sizeof(VInstr), 16);
-        cols_off = (uint32_t)off;
-        off = align_up(off + std::max<size_t>(s->in_types.size(), 1) * sizeof(ColIn), 16);
-        regs_off = (uint32_t)off;
-        off = align_up(off + (size_t)ns * T * 8, 16);
-        misc_off = (uint32_t)off;
-        off += 32 * 4 + (size_t)T * 4 + (size_t)(4 * (NT / 32)) * 8 + 16;  // s_cnt, exc_stage, look-back scratch, ticket
-        smem = (uint32_t)align_up(off, 16);
-        if (smem <= 72 * 1024 || (J == 2 && smem <= (uint32_t)d->smem_optin)) { Jsel = J; break; }
+        L = vec_layout(s, std::max<size_t>(n_uops, 1) * sizeof(VInstr), T, (size_t)ns * T * 8, true);
+        if (L.total <= 72 * 1024 || (J == 2 && L.total <= (uint32_t)d->smem_optin)) { Jsel = J; break; }
     }
-    // specialised K1v (jit.inl): the register file holds the live-out slots only; J = 4 (8 rows per thread) when that fits, else J = 2
+    // specialised kernels (jit.inl), whose register file holds the live-out slots only: K1r (nothing staged, the tile is evaluated
+    // again from L2 once its offset is known) for programs of a few operations; else K1w (4 sub-batches of 2048 rows per ticket) when
+    // the live-out slots fit the shared memory of 3 resident CTAs; else K1v with J = 4 (8 rows per thread) when that fits, else J = 2.
+    // While one of them is still compiling the interpreting kernel runs, and no second compile starts.
     jit::Loaded *jf = nullptr;
     if (jit_wanted(s, n)) {
         const uint32_t nl = std::max<uint32_t>((uint32_t)s->jit_live.slots.size(), 1);
-        const int forceJ = getenv("TPLX_JIT_VEC_J") ? atoi(getenv("TPLX_JIT_VEC_J")) : 0;  // experiments: tile size at equal occupancy
-        bool wide_pending = false;
-        // K1w (wide tiles: B sub-batches of 2048 rows per ticket) when the live-out slots of B sub-batches fit the shared memory of
-        // 3 (B = 4) / 4 (B = 2) resident CTAs; TPLX_JIT_WIDE=0 keeps K1v's 2048-row tiles
-        const int wide_max = getenv("TPLX_JIT_WIDE") ? atoi(getenv("TPLX_JIT_WIDE")) : 4;
-        // K1r (nothing staged, the tile is evaluated again from L2 once its offset is known) for programs of a few operations
-        const int re_b = getenv("TPLX_JIT_RE") ? atoi(getenv("TPLX_JIT_RE")) : 2;
-        const size_t re_max = getenv("TPLX_JIT_RE_MAX_INSTR") ? (size_t)atoi(getenv("TPLX_JIT_RE_MAX_INSTR")) : 16;
-        if (!forceJ && (re_b == 4 || re_b == 8 || re_b == 2 || re_b == 1) && s->instrs.size() <= re_max) {
-            const uint32_t Tw = (uint32_t)re_b * 2048u;
-            size_t off = 16;
-            const uint32_t c_off = (uint32_t)off;
-            off = align_up(off + std::max<size_t>(s->in_types.size(), 1) * sizeof(ColIn), 16);
-            const uint32_t r_off = (uint32_t)off;  // no register file
-            const uint32_t m_off = (uint32_t)off;
-            off += (size_t)re_b * 32 * 4 + (size_t)(4 * (NT / 32)) * 8 + 16;
-            const int kind = re_b == 4 ? jit::K_RE4 : (re_b == 8 ? jit::K_RE8 : (re_b == 2 ? jit::K_RE2 : jit::K_RE1));
+        bool pending = false;
+        auto take = [&](int kind, int J, uint32_t Tk, const Layout &Lk) {
             jf = jit_get(s, sd, kind, jit_minb(s, kind));
-            if (jf) { Jsel = 4; T = Tw; cols_off = c_off; regs_off = r_off; misc_off = m_off; smem = (uint32_t)align_up(off, 16); }
-            else if (jit_pending(s, kind)) wide_pending = true;
-        }
-        for (int Bw : {4, 2}) {
-            if (jf || wide_pending || forceJ || Bw > wide_max) continue;
-            const uint32_t Tw = (uint32_t)Bw * 2048u;
-            size_t off = 16;
-            const uint32_t c_off = (uint32_t)off;
-            off = align_up(off + std::max<size_t>(s->in_types.size(), 1) * sizeof(ColIn), 16);
-            const uint32_t r_off = (uint32_t)off;
-            off = align_up(off + (size_t)nl * Tw * 8, 16);
-            const uint32_t m_off = (uint32_t)off;
-            off += (size_t)Bw * 32 * 4 + (size_t)(4 * (NT / 32)) * 8 + 16;
-            if (align_up(off, 16) > (Bw == 4 ? 74u * 1024 : 55u * 1024)) continue;
-            const int kind = Bw == 4 ? jit::K_WIDE4 : jit::K_WIDE2;
-            jf = jit_get(s, sd, kind, jit_minb(s, kind));
-            if (jf) { Jsel = 4; T = Tw; cols_off = c_off; regs_off = r_off; misc_off = m_off; smem = (uint32_t)align_up(off, 16); }
-            else if (jit_pending(s, kind)) { wide_pending = true; break; }  // still compiling: interpreter meanwhile, no second compile
+            if (jf) { Jsel = J; T = Tk; L = Lk; }
+            else pending = jit_pending(s, kind);
+        };
+        if (s->instrs.size() <= 16) take(jit::K_RE2, 4, 2 * 2048u, vec_layout(s, 16, 2 * 2048u, 0, false));
+        if (!jf && !pending) {
+            const Layout Lw = vec_layout(s, 16, 4 * 2048u, (size_t)nl * 4 * 2048 * 8, false);
+            if (Lw.total <= 74u * 1024) take(jit::K_WIDE4, 4, 4 * 2048u, Lw);
         }
         for (int J : {4, 2}) {
-            if (jf || wide_pending) break;
-            if (forceJ && J != forceJ) continue;
+            if (jf || pending) break;
             const uint32_t Tj = 2u * J * NT;
-            size_t off = 16;
-            const uint32_t c_off = (uint32_t)off;
-            off = align_up(off + std::max<size_t>(s->in_types.size(), 1) * sizeof(ColIn), 16);
-            const uint32_t r_off = (uint32_t)off;
-            off = align_up(off + (size_t)nl * Tj * 8, 16);
-            const uint32_t m_off = (uint32_t)off;
-            off += 32 * 4 + (size_t)Tj * 4 + (size_t)(4 * (NT / 32)) * 8 + 16;
-            if (align_up(off, 16) > (J == 4 ? 56u * 1024 : 100u * 1024)) continue;
-            const int kind = J == 4 ? jit::K_VEC4 : jit::K_VEC2;
-            jf = jit_get(s, sd, kind, jit_minb(s, kind));
-            if (jf) { Jsel = J; T = Tj; cols_off = c_off; regs_off = r_off; misc_off = m_off; smem = (uint32_t)align_up(off, 16); }
+            const Layout Lj = vec_layout(s, 16, Tj, (size_t)nl * Tj * 8, true);
+            if (Lj.total > (J == 4 ? 56u * 1024 : 100u * 1024)) continue;
+            take(J == 4 ? jit::K_VEC4 : jit::K_VEC2, J, Tj, Lj);
             break;
         }
     }
     if (!Jsel) return TPLX_E_UNSUPPORTED;
+    const uint32_t smem = L.total;
     const int ji = Jsel == 4 ? 1 : 0;
     if (!jf && !sd->prog_vec[ji]) {
         std::lock_guard<std::mutex> lk(s->mu);
         if (!sd->prog_vec[ji]) {
-            std::vector<VInstr> dec = vec_encode(s->vplan, T, regs_off);
+            std::vector<VInstr> dec = vec_encode(s->vplan, T, L.regs_off);
             VInstr *p = nullptr;
             CU(cudaMalloc(&p, std::max<size_t>(dec.size() * sizeof(VInstr), 16)));
             CU(cudaMemcpy(p, dec.data(), dec.size() * sizeof(VInstr), cudaMemcpyHostToDevice));
             sd->prog_vec[ji] = reinterpret_cast<DInstr *>(p);
         }
     }
-    Layout L;
-    L.cols_off = cols_off;
-    L.regs_off = regs_off;
-    L.stage_off = regs_off;  // output columns are staged in place: a slot is indexed by the local row
-    L.misc_off = misc_off;
-    L.total = smem;
     KParams P;
     fill_common(P, s, sd, b, L, 2 * Jsel);
     P.prog = sd->prog_vec[ji];
@@ -1511,11 +1475,6 @@ static int32_t run_rows_vec(tplx_stage *s, StageDev *sd, const tplx_block *b, in
         if (rc) return rc;
     }
     P.cap_rows = n;
-    if (jf && getenv("TPLX_JIT_TIMES")) {  // diagnostic build of K1w: per-tile phase clocks
-        rc = dalloc(r, &P.tile_partials, (size_t)P.n_tiles * 8);
-        if (rc) return rc;
-        CU(cudaMemsetAsync(P.tile_partials, 0, (size_t)P.n_tiles * 64, d->stream));
-    }
     uint64_t cap_exc = std::max<uint64_t>(4096, (uint64_t)(s->est_exc_per_row * 1.5 * (double)n) + n / 64);
     for (int attempt = 0; attempt < 2; ++attempt) {
         P.cap_exc = cap_exc;
@@ -1542,11 +1501,6 @@ static int32_t run_rows_vec(tplx_stage *s, StageDev *sd, const tplx_block *b, in
         cap_exc = r->n_exc + 16;
     }
     CU(cudaEventRecord(r->evk1, d->stream));
-    if (P.tile_partials && getenv("TPLX_JIT_TIMES")) {
-        std::vector<uint64_t> h((size_t)P.n_tiles * 8);
-        CU(cudaMemcpy(h.data(), P.tile_partials, h.size() * 8, cudaMemcpyDeviceToHost));
-        if (FILE *f = fopen(getenv("TPLX_JIT_TIMES"), "wb")) { fwrite(h.data(), 8, h.size(), f); fclose(f); }
-    }
     for (size_t c = 0; c < s->out_cols.size(); ++c) r->out[c] = P.out[c];
     r->exc = P.exc;
     return TPLX_OK;
@@ -1594,23 +1548,21 @@ static int32_t run_rows(tplx_stage *s, StageDev *sd, const tplx_block *b, int64_
     if (jf) occ_regs = jit_occupancy(jf, 0);
     else CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_regs, stage_rows_kernel, NT, 0));
     occ_regs = std::max(occ_regs, 1);
-    const uint32_t env_R = getenv("TPLX_TILE_R") ? (uint32_t)atoi(getenv("TPLX_TILE_R")) : 0;
     uint32_t smem_budget = (uint32_t)(d->prop.sharedMemPerMultiprocessor / occ_regs) - 1024;
-    uint32_t R = env_R ? env_R : 16;
-    const bool allow_inplace = !(getenv("TPLX_NO_INPLACE") && atoi(getenv("TPLX_NO_INPLACE")));
+    uint32_t R = 16;
     Layout L = make_layout(s, R, true, false, jf != nullptr);
     while (R > 1 && L.total > smem_budget) {
         R /= 2;
-        L = make_layout(s, R, true, allow_inplace, jf != nullptr);  // one row per thread: no staging area, outputs are read from the register file
+        L = make_layout(s, R, true, true, jf != nullptr);  // one row per thread: no staging area, outputs are read from the register file
     }
     if (L.total > smem_budget && !(L.inplace && L.total <= (uint32_t)d->smem_optin)) {
         // even one row per thread does not fit the budget: give up occupancy instead
         smem_budget = (uint32_t)std::min<int>(d->smem_optin, 113 * 1024);
-        R = env_R ? env_R : 4;
+        R = 4;
         L = make_layout(s, R, true, false, jf != nullptr);
         while (R > 1 && L.total > smem_budget) {
             R /= 2;
-            L = make_layout(s, R, true, allow_inplace, jf != nullptr);
+            L = make_layout(s, R, true, true, jf != nullptr);
         }
     }
     if (L.total > (uint32_t)d->smem_optin) return fail(TPLX_E_UNSUPPORTED, "stage needs more shared memory than one SM has");
@@ -1620,9 +1572,8 @@ static int32_t run_rows(tplx_stage *s, StageDev *sd, const tplx_block *b, int64_
     if (occ < 1) return fail(TPLX_E_UNSUPPORTED, "stage kernel cannot be resident");
     // String stages read their input bytes through L1 again and again (every string op walks the bytes): shared memory must not
     // take the whole 256 KB of the SM's L1 / shared memory. The carve-out is capped at 196 KB (85 % of 228), which leaves 60 KB of
-    // L1 at 3 CTAs/SM, and occupancy is counted against it (TPLX_DENSE_CARVEOUT overrides the cap).
-    int carve = s->has_str ? 85 : -1;
-    if (getenv("TPLX_DENSE_CARVEOUT")) carve = atoi(getenv("TPLX_DENSE_CARVEOUT"));
+    // L1 at 3 CTAs/SM, and occupancy is counted against it.
+    const int carve = s->has_str ? 85 : -1;
     if (jf) jit::cudrv_api()->FuncSetAttribute(jf->fn, jit::CU_FUNC_ATTRIBUTE_PREFERRED_SHARED_MEMORY_CARVEOUT, carve);
     else CU(cudaFuncSetAttribute(stage_rows_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, carve));
     if (carve > 0 && carve < 100) {
@@ -1632,7 +1583,6 @@ static int32_t run_rows(tplx_stage *s, StageDev *sd, const tplx_block *b, int64_
             if (kb * 100 >= carve * 228) { cfg = kb; break; }
         occ = std::max(1, std::min(occ, (int)((size_t)cfg * 1024 / ((size_t)L.total + 1024))));
     }
-    if (getenv("TPLX_DENSE_OCC") && atoi(getenv("TPLX_DENSE_OCC")) > 0) occ = std::min(occ, atoi(getenv("TPLX_DENSE_OCC")));
     if (getenv("TPLX_TRACE"))
         fprintf(stderr, "[tplx] rows kernel%s: R %u, shared memory %u B (%s), %d CTAs/SM\n", jf ? " (specialised)" : "", R, L.total, L.inplace ? "in place" : "staged", occ);
     KParams P;
@@ -1640,9 +1590,6 @@ static int32_t run_rows(tplx_stage *s, StageDev *sd, const tplx_block *b, int64_
     if (jf) {
         P.n_instr = 0;
         P.n_slots = (uint32_t)s->jit_live.slots.size();
-        // dense-launch prefetch (jit_prefetch): on the Zillow dense launch it fetches whole 128-byte lines for cells that need one
-        // or two sectors, about twice the DRAM reads: off unless TPLX_JIT_PREFETCH=1
-        P.pad_split = (getenv("TPLX_JIT_PREFETCH") && atoi(getenv("TPLX_JIT_PREFETCH"))) ? 0u : 1u;
     }
     if (cols_override)
         for (size_t c = 0; c < cols_override->size(); ++c) P.in[c] = (*cols_override)[c];
@@ -1761,9 +1708,6 @@ static int32_t run_rows(tplx_stage *s, StageDev *sd, const tplx_block *b, int64_
 // no_wait: nothing here blocks the host — the survivor list gets the worst-case capacity (n rows), the exception records an
 // estimated one (*cap_exc_out), the counts stay on the device (*totals_dev: [0] survivors, [1] exception rows) and are also copied
 // into the lane's page-locked buffer in stream order; the caller reads them after its own synchronisation.
-#ifndef TPLX_MASK_MINB_DEFAULT
-#define TPLX_MASK_MINB_DEFAULT 4
-#endif
 static int32_t run_mask(tplx_stage *ps, StageDev *psd, const tplx_block *b, tplx_result *ra, bool no_wait, uint64_t **totals_dev, uint64_t *cap_exc_out) {
     Device *d = ra->dev;
     const uint64_t n = b->n_rows;
@@ -1785,13 +1729,12 @@ static int32_t run_mask(tplx_stage *ps, StageDev *psd, const tplx_block *b, tplx
     P.n_in = (uint32_t)ps->in_types.size();
     P.n_slots = std::max<uint32_t>(ps->hdr.n_slots, 1);
     // K1f: the planner stated the stage in closed form (string-scan hint) -> evaluate the terms directly, nothing is interpreted
-    bool scan = !ps->scan.empty() && !(getenv("TPLX_NO_SCAN") && atoi(getenv("TPLX_NO_SCAN")));
-    // specialised K1m (jit.inl): for prefilters without a closed form (TPLX_JIT_MASK=1: also instead of the closed form, to compare)
+    const bool scan = !ps->scan.empty() && !(getenv("TPLX_NO_SCAN") && atoi(getenv("TPLX_NO_SCAN")));
+    // specialised K1m (jit.inl): for prefilters without a closed form
     jit::Loaded *jf = nullptr;
-    if ((!scan || (getenv("TPLX_JIT_MASK") && atoi(getenv("TPLX_JIT_MASK")))) && jit_wanted(ps, n)) {
+    if (!scan && jit_wanted(ps, n)) {
         jf = jit_get(ps, psd, jit::K_MASK, jit_minb(ps, jit::K_MASK));
         if (jf) {
-            scan = false;
             P.n_slots = 0;  // no register file: nothing is live out of a prefilter program
             P.n_instr = 0;
         }
@@ -1802,79 +1745,27 @@ static int32_t run_mask(tplx_stage *ps, StageDev *psd, const tplx_block *b, tplx
         P.n_slots = 0;  // no register file
         P.n_instr = 0;
     }
-    P.MR = getenv("TPLX_MASK_MR") ? (uint32_t)std::max(1, std::min(4, atoi(getenv("TPLX_MASK_MR")))) : 1;
-    const uint32_t TR = 32 * P.MR;
-    P.n_tiles = (uint32_t)((n + TR - 1) / TR);
-    P.off_bytes = (uint32_t)align_up((TR + 1) * 4, 16);
+    P.n_tiles = (uint32_t)((n + 31) / 32);
     P.prog = psd->prog;
     P.cpool = psd->cpool;
     for (size_t c = 0; c < b->cols.size(); ++c) P.in[c] = b->cols[c];
-    // TPLX_MASK_STAGE=1: the string columns the program loads are staged through the warps' shared-memory rings (TMA bulk copies).
-    // The kernel is issue-bound rather than latency-bound: staging raises issue utilisation but its per-tile bookkeeping adds
-    // instructions, so plain coalesced loads through L1 are the default.
-    const bool want_stage = getenv("TPLX_MASK_STAGE") && atoi(getenv("TPLX_MASK_STAGE")) != 0;
-    std::vector<uint32_t> cand;
-    for (uint32_t i = 0; i < ps->instrs.size() && want_stage; ++i) {
-        const tplx_instr &in = ps->instrs[i];
-        if (in.op != TPLX_OP_LDCOL || in.flags != TPLX_T_STR) continue;
-        const uint32_t c = (uint32_t)in.imm;
-        if ((c < b->mapped.size() && b->mapped[c]) || (b->cols[c].type & COL_COMPACT)) continue;
-        if (std::find(cand.begin(), cand.end(), c) == cand.end()) cand.push_back(c);
-    }
-    const double slack = getenv("TPLX_MASK_SLACK") ? atof(getenv("TPLX_MASK_SLACK")) : 1.5;
-    auto cap_of = [&](uint32_t c) {
-        const double avg = (double)b->data_bytes[c] / (double)n;
-        return (uint32_t)std::min<uint64_t>(align_up((uint64_t)(avg * TR * slack) + 48, 16), 32768);
-    };
-    std::sort(cand.begin(), cand.end(), [&](uint32_t x, uint32_t y) { return cap_of(x) < cap_of(y); });
-    if (cand.size() > MASK_MAX_STAGED) cand.resize(MASK_MAX_STAGED);
-    uint32_t smem_total = 0;
-    const uint32_t smem_limit = getenv("TPLX_MASK_SMEM") ? (uint32_t)atoi(getenv("TPLX_MASK_SMEM")) : 72 * 1024;
-    for (;;) {  // drop the largest staged column until the CTA's shared memory fits the budget
-        P.n_staged = (uint32_t)cand.size();
-        uint32_t so = 0;
-        for (uint32_t k = 0; k < P.n_staged; ++k) {
-            P.st_col[k] = cand[k];
-            P.st_cap[k] = cap_of(cand[k]);
-            P.st_boff[k] = so;
-            so += P.st_cap[k];
-            P.st_ooff[k] = so;
-            so += P.off_bytes;
-        }
-        P.slot_bytes = (uint32_t)align_up(so, 128);
-        size_t off = align_up(std::max<size_t>(P.n_instr, 1) * sizeof(DInstr), 16);
-        P.smem_regs_off = (uint32_t)off;
-        off = align_up(off + (size_t)P.n_slots * NT * 8, 16);
-        P.smem_wcols_off = (uint32_t)off;
-        off = align_up(off + (size_t)MASK_WARPS * std::max<uint32_t>(P.n_in, 1) * sizeof(ColIn), 16);
-        P.smem_bar_off = (uint32_t)off;
-        off += MASK_WARPS * MASK_RING * 8;
-        P.smem_info_off = (uint32_t)off;
-        off = align_up(off + MASK_WARPS * MASK_RING * 2 * MASK_MAX_STAGED * 4, 128);
-        P.smem_ring_off = (uint32_t)off;
-        off += (size_t)MASK_WARPS * MASK_RING * P.slot_bytes;
-        smem_total = (uint32_t)off;
-        if (smem_total <= smem_limit || cand.empty()) break;
-        cand.pop_back();
-    }
+    size_t off = align_up(std::max<size_t>(P.n_instr, 1) * sizeof(DInstr), 16);
+    P.smem_regs_off = (uint32_t)off;
+    off = align_up(off + (size_t)P.n_slots * NT * 8, 16);
+    P.smem_cols_off = (uint32_t)off;
+    const uint32_t smem_total = (uint32_t)align_up(off + std::max<uint32_t>(P.n_in, 1) * sizeof(ColIn), 16);
     if (smem_total > (uint32_t)d->smem_optin) return fail(TPLX_E_UNSUPPORTED, "mask stage needs more shared memory than one SM has");
     int occ = 0;
-    // closed-form kernel: register budget per thread traded for resident warps (TPLX_MASK_MINB = 4 | 5 | 6 CTAs per SM)
-    const int minb = getenv("TPLX_MASK_MINB") ? atoi(getenv("TPLX_MASK_MINB")) : TPLX_MASK_MINB_DEFAULT;
     if (jf) occ = jit_occupancy(jf, smem_total);
-    else if (scan && minb == 6) CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, stage_mask_kernel<true, 6>, NT, smem_total));
-    else if (scan && minb == 5) CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, stage_mask_kernel<true, 5>, NT, smem_total));
-    else if (scan) CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, stage_mask_kernel<true, 4>, NT, smem_total));
+    else if (scan) CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, stage_mask_kernel<true>, NT, smem_total));
     else CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, stage_mask_kernel<false>, NT, smem_total));
     if (occ < 1) return fail(TPLX_E_UNSUPPORTED, "mask kernel cannot be resident");
-    // TPLX_MASK_OCC caps the resident CTAs per SM: leaving registers free lets the dense launch of another block (other lane) co-reside
-    if (getenv("TPLX_MASK_OCC")) occ = std::max(1, std::min(occ, atoi(getenv("TPLX_MASK_OCC"))));
     const uint32_t grid = std::max<uint32_t>(1, std::min<uint32_t>((P.n_tiles + MASK_WARPS - 1) / MASK_WARPS, (uint32_t)(occ * d->prop.multiProcessorCount)));
     P.scratch_per_thread = ps->materialises ? std::max<uint32_t>(ps->hdr.scratch_bytes, 64) : 0;
     int32_t rc = ensure_scratch(d, (size_t)grid * NT * P.scratch_per_thread);
     if (rc) return rc;
     P.scratch = d->scratch;
-    const uint32_t n_words = P.n_tiles * P.MR;
+    const uint32_t n_words = P.n_tiles;
     const uint32_t nb = (n_words + CMP_NT - 1) / CMP_NT;
     uint64_t *part = nullptr, *totals = nullptr;
     rc = dalloc(ra, &P.keep_words, n_words);
@@ -1891,9 +1782,7 @@ static int32_t run_mask(tplx_stage *ps, StageDev *psd, const tplx_block *b, tplx
         rc = jit_launch(jf, grid, smem_total, d->stream, &P);
         if (rc) return rc;
         ra->jit_launches += 1;
-    } else if (scan && minb == 6) stage_mask_kernel<true, 6><<<grid, NT, smem_total, d->stream>>>(P);
-    else if (scan && minb == 5) stage_mask_kernel<true, 5><<<grid, NT, smem_total, d->stream>>>(P);
-    else if (scan) stage_mask_kernel<true, 4><<<grid, NT, smem_total, d->stream>>>(P);
+    } else if (scan) stage_mask_kernel<true><<<grid, NT, smem_total, d->stream>>>(P);
     else stage_mask_kernel<false><<<grid, NT, smem_total, d->stream>>>(P);
     CU(cudaGetLastError());
     mask_count_kernel<<<nb, CMP_NT, 0, d->stream>>>(P.keep_words, P.exc_words, n_words, part);
@@ -1961,15 +1850,14 @@ static int32_t run_rows_prefiltered(tplx_stage *s, StageDev *sd, const tplx_bloc
         decltype(drop_ra) &f;
         ~OnExit() { f(); }
     } ra_guard{drop_ra};
-    const bool use_mask = !(getenv("TPLX_NO_MASK") && atoi(getenv("TPLX_NO_MASK")));
     bool any_mapped = false;
     for (uint8_t m : b->mapped) any_mapped = any_mapped || m;
     // Steady state without a host round trip between the two launches: once a block has shown the selectivity, the dense launch of
     // the next block is sized from it (x1.3 + slack) and reads the real survivor count on the device; the host synchronises once,
     // at the end. (Blocks with late columns in host memory size their gather from the exact count and keep the round trip.)
-    const bool no_wait = use_mask && !any_mapped && ps->est_surv_ratio >= 0.0 && b->n_rows > 0 && !(getenv("TPLX_SYNC_PREFILTER") && atoi(getenv("TPLX_SYNC_PREFILTER")));
+    const bool no_wait = !any_mapped && ps->est_surv_ratio >= 0.0 && b->n_rows > 0 && !(getenv("TPLX_SYNC_PREFILTER") && atoi(getenv("TPLX_SYNC_PREFILTER")));
     uint64_t *totals_dev = nullptr, cap_exc_a = 0;
-    rc = use_mask ? run_mask(ps, psd, b, &ra, no_wait, &totals_dev, &cap_exc_a) : run_rows(ps, psd, b, 0, &ra, nullptr, 0);
+    rc = run_mask(ps, psd, b, &ra, no_wait, &totals_dev, &cap_exc_a);
     if (rc) { drop_ra(); return rc; }
     // the prefilter's kernel interval is timed lazily (result_info): no host synchronisation for it here
     r->extra_ev.emplace_back(ra.evk0, ra.evk1);
@@ -2005,7 +1893,7 @@ static int32_t run_rows_prefiltered(tplx_stage *s, StageDev *sd, const tplx_bloc
     }
     const uint64_t n_surv = ra.n_out;
     if (!no_wait) {
-        if (b->n_rows) { ps->est_surv_ratio = (double)n_surv / (double)b->n_rows; if (use_mask) ps->est_exc_per_row = (double)ra.n_exc / (double)b->n_rows; }
+        if (b->n_rows) { ps->est_surv_ratio = (double)n_surv / (double)b->n_rows; ps->est_exc_per_row = (double)ra.n_exc / (double)b->n_rows; }
     }
     if (b->n_rows >= (1u << 16) && n_surv * 2 > b->n_rows) s->prefilter_enabled = false;  // not selective: stop using it
     // late columns that still live in host memory: bring over the surviving rows only (gather.cuh)

@@ -408,26 +408,20 @@ __device__ __forceinline__ void jit_eval_vec(const ulonglong2 (&vin)[J][JIT_NIN]
 }
 #endif
 
-#ifdef TPLX_JIT_TIMES
-#define TPLX_TQ(i) tq[i] = clock64()
-#else
-#define TPLX_TQ(i)
-#endif
-
-#if defined(TPLX_JIT) && (TPLX_JIT_KIND == 6 || TPLX_JIT_KIND == 7)
+#if defined(TPLX_JIT) && TPLX_JIT_KIND == 6
 // ---- K1w: the specialised fixed-width row kernel with WIDE tiles ---------------------------------------------------------------------
 // On C1, with the interpretation gone, K1v is bound by the latency chain of a tile — ticket, LDG,
 // counts, look-back over every earlier tile still in flight, stores — of which the look-back waits for the SLOWEST load among all
 // predecessors (in-order retirement over a window of ~1000 tiles), however few instructions the tile takes.
-// Only resident warps hide that, and a specialised row function leaves registers and shared memory to spare. So a CTA takes B = 4 (or 2)
+// Only resident warps hide that, and a specialised row function leaves registers and shared memory to spare. So a CTA takes B = 4
 // sub-batches of 2048 rows per ticket: one ticket, one count barrier, ONE look-back and one inclusive-prefix publication per 8192 rows,
 // 64 KB of loads per CTA between two waits; the sub-batches are evaluated back to back (the LDG.128s of sub-batch b + 1 are issued before
 // sub-batch b is evaluated when the registers allow), their live-out slots staged side by side in the compact register file
 // (regs[slot][b][local row]), exception codes of raising rows in slot 0 of that row (a raising row is not written).
 // Same row order, same packed tile-state word, same output as K1v with tiles four times the size.
-extern "C" __global__ void __launch_bounds__(NT, TPLX_JIT_MINB) tplx_jit_kernel(const __grid_constant__ KParams P) {
+extern "C" __global__ void __launch_bounds__(NT, TPLX_JIT_MIN_CTAS) tplx_jit_kernel(const __grid_constant__ KParams P) {
     extern __shared__ __align__(16) uint8_t smem[];
-    constexpr int J = 4, B = TPLX_JIT_KIND == 6 ? 4 : 2;
+    constexpr int J = 4, B = 4;
     using VV = VecVM<J>;
     constexpr uint32_t TS = VV::T, T = B * TS, SLOT_W = T * 8;  // rows per sub-batch / per tile, bytes of one slot of the wide register file
     const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -452,10 +446,6 @@ extern "C" __global__ void __launch_bounds__(NT, TPLX_JIT_MINB) tplx_jit_kernel(
         const uint32_t tile = s_ctl[0];
         if (tile >= P.n_tiles) break;
         const uint64_t base = (uint64_t)tile * T;
-#ifdef TPLX_JIT_TIMES  // diagnostic build (TPLX_JIT_TIMES=<file>): thread 0's clock at the phase boundaries of every tile
-        long long tq[6];
-        tq[0] = clock64();
-#endif
 
         // ---- evaluate the B sub-batches ----
         uint32_t alive[B], excb[B];
@@ -510,7 +500,6 @@ extern "C" __global__ void __launch_bounds__(NT, TPLX_JIT_MINB) tplx_jit_kernel(
             }
         }
 
-        TPLX_TQ(1);
         // ---- counts per (sub-batch, slab, warp) group ----
         uint32_t any_exc = 0;
 #pragma unroll
@@ -548,10 +537,8 @@ extern "C" __global__ void __launch_bounds__(NT, TPLX_JIT_MINB) tplx_jit_kernel(
         if (tid == 0)  // publish this tile's counts (tile 0: they are its inclusive prefix)
             st_cg_u64(P.tile_state + tile, ((uint64_t)(tile == 0 ? 2u : 1u) << 62) | ((uint64_t)n_keep << 31) | (uint64_t)n_exc);
 
-        TPLX_TQ(2);
         uint64_t pre_keep = 0, pre_exc = 0;
         vec_lookback(P, tile, n_keep, n_exc, s_scr, pre_keep, pre_exc);
-        TPLX_TQ(3);
         if (tid == 0 && tile == P.n_tiles - 1) {
             P.totals[0] = pre_keep + n_keep;
             P.totals[1] = pre_exc + n_exc;
@@ -598,26 +585,15 @@ extern "C" __global__ void __launch_bounds__(NT, TPLX_JIT_MINB) tplx_jit_kernel(
                 }
             }
         }
-        TPLX_TQ(4);
         if (tid == 0) s_ctl[0] = atomicAdd(&P.counters[0], 1u);  // every thread read the old ticket before the counts barrier of this tile
-#ifdef TPLX_JIT_TIMES
-        if (tid == 0 && P.tile_partials) {
-            tq[5] = clock64();
-            uint32_t smid;
-            asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
-            for (int i = 0; i < 6; ++i) P.tile_partials[(size_t)tile * 8 + i] = (uint64_t)tq[i];
-            P.tile_partials[(size_t)tile * 8 + 6] = smid;
-            P.tile_partials[(size_t)tile * 8 + 7] = blockIdx.x;
-        }
-#endif
     }
 }
 #endif  // K1w
 
-#if defined(TPLX_JIT) && (TPLX_JIT_KIND >= 8 && TPLX_JIT_KIND <= 11)
+#if defined(TPLX_JIT) && TPLX_JIT_KIND == 10
 // ---- K1r: the specialised fixed-width row kernel that stages NOTHING: L2 is the staging buffer ----------------------------------------
-// Per-tile phase clocks of K1w on C1 (tools/tile_times.py): load + evaluate, counts, look-back (= waiting for the slowest load among the
-// ~1000 tiles in flight: in-order retirement), stores. Rows sit in shared memory from their evaluation to their store, and shared memory
+// A tile of K1w goes through four phases: load + evaluate, counts, look-back (= waiting for the slowest load among the ~1000 tiles
+// in flight: in-order retirement), stores. Rows sit in shared memory from their evaluation to their store, and shared memory
 // bounds the rows in flight (132 SMs x 227 KB / 8 B = 3.8 M rows on H100): throughput = rows in flight / latency. Short of making DRAM
 // latency deterministic, the way out is to hold rows in flight somewhere bigger: the 50 MB L2. K1r evaluates a tile TWICE:
 //   pass 1: LDG.128 the inputs, run the row function for the row's FATE only (kept / filtered / raised: two bits per row in registers),
@@ -629,9 +605,9 @@ extern "C" __global__ void __launch_bounds__(NT, TPLX_JIT_MINB) tplx_jit_kernel(
 // CTA can keep TWO tiles in flight for the price of ten registers: the look-back of tile A (the wait for the slowest of its predecessors)
 // is done after pass 1 of the CTA's next tile B has been issued and B's counts are published — the wait overlaps real work, and no
 // ticket is ever held without its counts being produced as fast as the CTA can.
-extern "C" __global__ void __launch_bounds__(NT, TPLX_JIT_MINB) tplx_jit_kernel(const __grid_constant__ KParams P) {
+extern "C" __global__ void __launch_bounds__(NT, TPLX_JIT_MIN_CTAS) tplx_jit_kernel(const __grid_constant__ KParams P) {
     extern __shared__ __align__(16) uint8_t smem[];
-    constexpr int J = 4, B = TPLX_JIT_KIND == 8 ? 4 : (TPLX_JIT_KIND == 9 ? 8 : (TPLX_JIT_KIND == 10 ? 2 : 1));
+    constexpr int J = 4, B = 2;
     using VV = VecVM<J>;
     constexpr uint32_t TS = VV::T, T = B * TS;
     const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -691,7 +667,7 @@ extern "C" __global__ void __launch_bounds__(NT, TPLX_JIT_MINB) tplx_jit_kernel(
             }
         }
         __syncthreads();
-        uint32_t run = 0;  // kept in the low half, raised in the high half: both <= T = 16384 < 2^16
+        uint32_t run = 0;  // kept in the low half, raised in the high half: both <= T = 4096 < 2^16
 #pragma unroll
         for (uint32_t b = 0; b < B; ++b) {
             uint32_t gi = s_cnt[b * 32 + lane];
@@ -779,10 +755,7 @@ extern "C" __global__ void __launch_bounds__(NT, TPLX_JIT_MINB) tplx_jit_kernel(
     };
 
     // Two tiles in flight per CTA: pass 1 of the new ticket first (its counts are what every successor waits for), then the
-    // look-back + pass 2 of the previous one. TPLX_JIT_DEFER 0: one tile at a time.
-#ifndef TPLX_JIT_DEFER
-#define TPLX_JIT_DEFER 1
-#endif
+    // look-back + pass 2 of the previous one.
     Tile cur, prev;
     bool have_prev = false;
     if (tid == 0) s_ctl[0] = atomicAdd(&P.counters[0], 1u);
@@ -791,15 +764,10 @@ extern "C" __global__ void __launch_bounds__(NT, TPLX_JIT_MINB) tplx_jit_kernel(
         cur.tile = s_ctl[0];
         const bool have = cur.tile < P.n_tiles;  // uniform
         if (have) first_pass(cur);
-        if (TPLX_JIT_DEFER) {
-            if (have_prev) second_pass(prev);
-            if (!have) break;
-            prev = cur;
-            have_prev = true;
-        } else {
-            if (!have) break;
-            second_pass(cur);
-        }
+        if (have_prev) second_pass(prev);
+        if (!have) break;
+        prev = cur;
+        have_prev = true;
         if (tid == 0) s_ctl[0] = atomicAdd(&P.counters[0], 1u);  // every thread has read the old ticket (barrier of first_pass)
     }
 }
@@ -807,7 +775,7 @@ extern "C" __global__ void __launch_bounds__(NT, TPLX_JIT_MINB) tplx_jit_kernel(
 
 #if !defined(TPLX_JIT) || TPLX_JIT_KIND == 2 || TPLX_JIT_KIND == 3
 #ifdef TPLX_JIT
-extern "C" __global__ void __launch_bounds__(NT, TPLX_JIT_MINB) tplx_jit_kernel(const __grid_constant__ KParams P) {
+extern "C" __global__ void __launch_bounds__(NT, TPLX_JIT_MIN_CTAS) tplx_jit_kernel(const __grid_constant__ KParams P) {
     constexpr int J = TPLX_JIT_KIND == 3 ? 2 : 4;
 #else
 template <int J>
