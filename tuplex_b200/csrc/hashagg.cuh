@@ -11,6 +11,7 @@
 #pragma once
 #include <stdint.h>
 #include "kernels.cuh"
+#include "keyhash.cuh"
 
 namespace tplx {
 
@@ -43,11 +44,6 @@ struct HashParams {
     uint32_t *overflow_rows;   // rows whose key could not be inserted (table/heap full)
     uint64_t cap_overflow;
 };
-
-__device__ __forceinline__ uint64_t mix64(uint64_t x) {
-    x ^= x >> 33; x *= 0xff51afd7ed558ccdull; x ^= x >> 33; x *= 0xc4ceb9fe1a85ec53ull; x ^= x >> 33;
-    return x;
-}
 
 template <int NTT>
 __device__ __forceinline__ uint64_t hash_key(const HashParams &H, uint8_t *regs, uint32_t *blob_size) {

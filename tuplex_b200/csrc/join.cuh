@@ -27,7 +27,7 @@
 #pragma once
 #include <stdint.h>
 #include "kernels.cuh"
-#include "hashagg.cuh"
+#include "keyhash.cuh"
 
 namespace tplx {
 
@@ -59,12 +59,9 @@ __device__ __forceinline__ bool join_is_null(const JoinKey &k, uint64_t r) {
 __device__ __forceinline__ uint64_t join_hash(const JoinKey &k, uint64_t r) {
     if (k.type == TPLX_T_STR) {
         const uint32_t o0 = k.offsets[r], o1 = k.offsets[r + 1];
-        const uint8_t *p = reinterpret_cast<const uint8_t *>(k.data) + o0;
-        uint64_t f = 0xcbf29ce484222325ull;
-        for (uint32_t i = 0; i < o1 - o0; ++i) f = (f ^ p[i]) * 0x100000001b3ull;
-        return mix64(f ^ ((uint64_t)(o1 - o0) << 48));
+        return key_hash_bytes(reinterpret_cast<const uint8_t *>(k.data) + o0, o1 - o0);
     }
-    return mix64(reinterpret_cast<const uint64_t *>(k.data)[r] ^ 0x9E3779B97F4A7C15ull);
+    return key_hash_i64(reinterpret_cast<const uint64_t *>(k.data)[r]);
 }
 
 __device__ __forceinline__ bool join_key_equal(const JoinKey &a, uint64_t ra, const JoinKey &b, uint64_t rb) {
