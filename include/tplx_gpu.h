@@ -194,7 +194,9 @@ int32_t tplx_gpu_result_free(tplx_result *res);
 int32_t tplx_gpu_stage_hash_reserve(tplx_stage *stage, int32_t device, uint64_t expected_keys);
 int32_t tplx_gpu_stage_hash_finish(tplx_stage *stage, int32_t device, tplx_result **out);
 /* Merge packed (key columns, accumulator columns) rows — e.g. received from another GPU over
- * NCCL — into this device's table using the accumulators' combine operation. */
+ * NCCL — into this device's table using the accumulators' combine operation. A key column that is
+ * an Option key of the stage may carry a validity bitmap (tplx_column.valid; no bitmap = no None);
+ * a bitmap on any other column is rejected. */
 int32_t tplx_gpu_stage_hash_merge(tplx_stage *stage, const tplx_block *packed);
 /* Like hash_finish but the accumulator columns hold raw partials (initial value not applied): the form
  * that is exchanged between GPUs before the owner of a key range merges and finishes. */

@@ -204,7 +204,11 @@ typedef struct tplx_outcol {
     uint16_t slot;   /* value slot at program end */
     uint8_t type;    /* tplx_type */
     uint8_t null_of; /* 0, or 1 + k: this (hidden, TPLX_T_BOOL) column is 1 where output column k — an Option[T] column — holds None;
-                        the executor turns it into column k's validity bitmap (tplx_gpu_result_fetch_validity) */
+                        the executor turns it into column k's validity bitmap (tplx_gpu_result_fetch_validity).
+                        HASH endpoint: allowed on hidden bool columns behind the keys only, and k must be one of the first n_keys
+                        columns (at most one companion per key). Rows whose flag is 1 form key k's None group: the key's value
+                        slot is then ignored, None differs from every value (0, "", False), and the hash result carries
+                        the key column with a validity bitmap (placeholder 0 / "" under None). */
 } tplx_outcol;
 
 typedef struct tplx_acc {
@@ -326,7 +330,8 @@ typedef struct tplx_stage_header {
     uint16_t n_in_cols;
     uint16_t n_out_cols;
     uint16_t n_accs;
-    uint16_t n_keys;      /* HASH endpoint: first n_keys out_cols are the key */
+    uint16_t n_keys;      /* HASH endpoint: first n_keys out_cols are the key; hidden `is None` companions of Option keys
+                             (tplx_outcol.null_of) may follow them */
     uint16_t n_ops;
     uint16_t n_slots;     /* register file size in 8-byte slots */
     uint32_t n_instr;

@@ -479,7 +479,7 @@ class Result:
         p = self.stage.program
         if self.hash_result:
             f = {ir.C["TPLX_ACC_SUM_F64"], ir.C["TPLX_ACC_MIN_F64"], ir.C["TPLX_ACC_MAX_F64"]}
-            return [t for _, t in p.out_cols] + [T_F64 if a.kind in f else T_I64 for a in p.accs]
+            return [t for _, t in p.out_cols[: p.n_keys]] + [T_F64 if a.kind in f else T_I64 for a in p.accs]
         return [t for _, t in p.out_cols][: len(p.out_cols) - p.hidden_out_cols]
 
     def column(self, c: int) -> Column:

@@ -23,7 +23,8 @@ struct HashTableDev {
     uint64_t *state;    // 0 empty, 1 busy, else fingerprint (hash | 2)
     uint64_t *keyoff;   // heap offset | blob size << 40
     uint64_t *accs;     // [n_accs][cap]
-    uint8_t *heap;      // key blobs: per key column i64 -> 8 bytes, str -> u32 len + bytes
+    uint8_t *heap;      // key blobs: per key column i64 -> 8 bytes, str -> u32 len + bytes; an Option key column puts one flag
+                        // byte in front (1 = None, and then nothing follows; 0 = the value's encoding follows)
     uint64_t cap, mask, max_keys, heap_cap;
     uint64_t *counters; // [0] n_keys, [1] heap_used, [2] overflow rows, [3] exception append
 };
@@ -39,17 +40,33 @@ struct HashParams {
     uint32_t n_keys;
     uint32_t key_slot[TPLX_MAX_KEYS];
     uint32_t key_type[TPLX_MAX_KEYS];
+    uint32_t key_null[TPLX_MAX_KEYS];  // slot of key k's "is None" flag, TPLX_NOSLOT when key k cannot be None
     const uint32_t *rowlist;   // optional: process these rows only (overflow retry)
     uint64_t n_list;
     uint32_t *overflow_rows;   // rows whose key could not be inserted (table/heap full)
     uint64_t cap_overflow;
 };
 
+// A None key is one group whatever its value slot holds (the other branch of a select, junk under an invalid input row): the slot
+// is never read for it, so it reaches neither the hash nor the comparison nor the blob. OPT: the stage has Option keys (a stage
+// without them runs code in which none of these tests exist).
 template <int NTT>
+__device__ __forceinline__ bool key_is_none(const HashParams &H, uint8_t *regs, uint32_t k) {
+    return H.key_null[k] != TPLX_NOSLOT && VM<NTT>::R(regs, H.key_null[k] * VM<NTT>::SLOT_BYTES) != 0;
+}
+
+template <int NTT, bool OPT>
 __device__ __forceinline__ uint64_t hash_key(const HashParams &H, uint8_t *regs, uint32_t *blob_size) {
     uint64_t h = 0x9E3779B97F4A7C15ull;
     uint32_t sz = 0;
     for (uint32_t k = 0; k < H.n_keys; ++k) {
+        if (OPT && H.key_null[k] != TPLX_NOSLOT) {
+            sz += 1;
+            if (key_is_none<NTT>(H, regs, k)) {
+                h = mix64(h ^ 0x4E6F6E654B657921ull);
+                continue;
+            }
+        }
         if (H.key_type[k] == TPLX_T_STR) {
             StrV s = VM<NTT>::RS(regs, H.key_slot[k] * VM<NTT>::SLOT_BYTES);
             uint64_t f = 0xcbf29ce484222325ull;
@@ -65,9 +82,14 @@ __device__ __forceinline__ uint64_t hash_key(const HashParams &H, uint8_t *regs,
     return h;
 }
 
-template <int NTT>
+template <int NTT, bool OPT>
 __device__ __forceinline__ bool key_equal(const HashParams &H, uint8_t *regs, const uint8_t *blob) {
     for (uint32_t k = 0; k < H.n_keys; ++k) {
+        if (OPT && H.key_null[k] != TPLX_NOSLOT) {
+            const bool none = key_is_none<NTT>(H, regs, k);
+            if ((*blob++ != 0) != none) return false;
+            if (none) continue;
+        }
         if (H.key_type[k] == TPLX_T_STR) {
             StrV s = VM<NTT>::RS(regs, H.key_slot[k] * VM<NTT>::SLOT_BYTES);
             uint32_t len = blob[0] | (blob[1] << 8) | (blob[2] << 16) | ((uint32_t)blob[3] << 24);
@@ -86,9 +108,14 @@ __device__ __forceinline__ bool key_equal(const HashParams &H, uint8_t *regs, co
     return true;
 }
 
-template <int NTT>
+template <int NTT, bool OPT>
 __device__ __forceinline__ void key_write(const HashParams &H, uint8_t *regs, uint8_t *blob) {
     for (uint32_t k = 0; k < H.n_keys; ++k) {
+        if (OPT && H.key_null[k] != TPLX_NOSLOT) {
+            const bool none = key_is_none<NTT>(H, regs, k);
+            *blob++ = none ? 1 : 0;
+            if (none) continue;
+        }
         if (H.key_type[k] == TPLX_T_STR) {
             StrV s = VM<NTT>::RS(regs, H.key_slot[k] * VM<NTT>::SLOT_BYTES);
             blob[0] = (uint8_t)s.len; blob[1] = (uint8_t)(s.len >> 8); blob[2] = (uint8_t)(s.len >> 16); blob[3] = (uint8_t)(s.len >> 24);
@@ -113,7 +140,7 @@ __device__ __forceinline__ void st_release_u64(uint64_t *p, uint64_t v) {
 }
 
 // returns table slot of the key, inserting it if absent; HT_NOT_FOUND when the table or heap is full
-template <int NTT>
+template <int NTT, bool OPT>
 __device__ uint32_t find_or_insert(const HashParams &H, uint8_t *regs, uint64_t h, uint32_t blob_size) {
     const HashTableDev &T = H.ht;
     const uint64_t fp = h | 2ull;
@@ -137,7 +164,7 @@ __device__ uint32_t find_or_insert(const HashParams &H, uint8_t *regs, uint64_t 
                         st_release_u64(&T.state[idx], 0ull);
                         return HT_NOT_FOUND;
                     }
-                    key_write<NTT>(H, regs, T.heap + off);
+                    key_write<NTT, OPT>(H, regs, T.heap + off);
                     T.keyoff[idx] = off | ((uint64_t)blob_size << 40);
                     __threadfence();
                     st_release_u64(&T.state[idx], fp);
@@ -151,7 +178,7 @@ __device__ uint32_t find_or_insert(const HashParams &H, uint8_t *regs, uint64_t 
         if (st == fp) {
             __threadfence();
             const uint64_t ko = ld_cg_u64(&T.keyoff[idx]);
-            if ((uint32_t)(ko >> 40) == blob_size && key_equal<NTT>(H, regs, T.heap + (ko & ((1ull << 40) - 1)))) return (uint32_t)idx;
+            if ((uint32_t)(ko >> 40) == blob_size && key_equal<NTT, OPT>(H, regs, T.heap + (ko & ((1ull << 40) - 1)))) return (uint32_t)idx;
         }
         idx = (idx + 1) & T.mask;
     }
@@ -187,9 +214,9 @@ __global__ void hash_init_accs(HashTableDev T, uint32_t n_accs, const AccP *accs
 // =============================================================================================
 // K4: rows in -> hash table.  Same tile/VM structure as K3; the per-row sink is the table.
 // EXC_ONLY: collect the exception records only and leave the table alone (second pass over a block whose exception rows did
-// not fit the first pass's buffer).
+// not fit the first pass's buffer). OPT_KEYS: some key column can be None (HashParams.key_null).
 // =============================================================================================
-template <bool EXC_ONLY>
+template <bool EXC_ONLY, bool OPT_KEYS>
 __global__ void __launch_bounds__(NT) stage_hash_kernel(const KParams *__restrict__ Pg, const HashParams *__restrict__ Hg) {
     extern __shared__ __align__(16) uint8_t smem[];
     const KParams &P = *Pg;
@@ -236,8 +263,8 @@ __global__ void __launch_bounds__(NT) stage_hash_kernel(const KParams *__restric
             VM<NT>::run(s_prog, 0, P.n_instr, s_regs, s_cols, row, row, P.cpool, t);
             if (!EXC_ONLY && t.alive) {
                 uint32_t blob = 0;
-                const uint64_t h = hash_key<NT>(H, s_regs, &blob);
-                const uint32_t g = find_or_insert<NT>(H, s_regs, h, blob);
+                const uint64_t h = hash_key<NT, OPT_KEYS>(H, s_regs, &blob);
+                const uint32_t g = find_or_insert<NT, OPT_KEYS>(H, s_regs, h, blob);
                 if (g == HT_NOT_FOUND) {
                     uint64_t pos = atomicAdd((unsigned long long *)&H.ht.counters[2], 1ull);
                     if (pos < H.cap_overflow) H.overflow_rows[pos] = (uint32_t)row;
@@ -339,33 +366,36 @@ __global__ void hash_flag_slots(HashTableDev T, uint64_t *flags, HashSel sel) {
     uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < T.cap) flags[i] = slot_selected(T.state[i], sel) ? 1 : 0;
 }
-// ... per-key string lengths of key column kc at compacted position (for the per-column offset scan)
-__global__ void hash_key_lens(HashTableDev T, const uint64_t *pos, uint32_t n_keys, const uint32_t *key_types, uint32_t kc,
-                              uint64_t *lens, HashSel sel) {
-    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= T.cap || !slot_selected(T.state[i], sel)) return;
-    const uint8_t *blob = T.heap + (T.keyoff[i] & ((1ull << 40) - 1));
-    for (uint32_t k = 0; k < kc; ++k) {
-        if (key_types[k] == TPLX_T_STR) {
-            uint32_t len = blob[0] | (blob[1] << 8) | (blob[2] << 16) | ((uint32_t)blob[3] << 24);
-            blob += 4 + len;
-        } else blob += 8;
-    }
-    uint32_t len = blob[0] | (blob[1] << 8) | (blob[2] << 16) | ((uint32_t)blob[3] << 24);
-    lens[pos[i]] = len;
-}
 struct HashEmit {
     uint32_t n_keys, n_accs;
     uint32_t key_types[TPLX_MAX_KEYS];
     uint32_t acc_kinds[TPLX_MAX_ACCS];
     int64_t acc_init[TPLX_MAX_ACCS];
+    uint64_t *key_none[TPLX_MAX_KEYS];     // Option key columns: 1 where the group's key is None (packed into the validity bitmap
+                                           // afterwards); nullptr for a key column that cannot be None
     uint64_t *key_data[TPLX_MAX_KEYS];     // i64 keys
     uint32_t *key_offsets[TPLX_MAX_KEYS];  // str keys: offsets (n+1)
     const uint64_t *key_lens_scan[TPLX_MAX_KEYS];  // exclusive byte offsets per compacted key (n+1)
     uint8_t *key_bytes[TPLX_MAX_KEYS];
     uint64_t *acc_data[TPLX_MAX_ACCS];
 };
-// ... and emit key + accumulator columns at the compacted position
+__device__ __forceinline__ uint32_t blob_u32(const uint8_t *p) { return p[0] | (p[1] << 8) | (p[2] << 16) | ((uint32_t)p[3] << 24); }
+// steps over the flag byte of an Option key column; true when the key is None (no value follows)
+__device__ __forceinline__ bool blob_none(const uint8_t *&blob, const HashEmit &E, uint32_t k) {
+    return E.key_none[k] && *blob++ != 0;
+}
+// ... per-key string lengths of key column kc at compacted position (for the per-column offset scan; 0 for a None key)
+__global__ void hash_key_lens(HashTableDev T, const uint64_t *pos, HashEmit E, uint32_t kc, uint64_t *lens, HashSel sel) {
+    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= T.cap || !slot_selected(T.state[i], sel)) return;
+    const uint8_t *blob = T.heap + (T.keyoff[i] & ((1ull << 40) - 1));
+    for (uint32_t k = 0; k < kc; ++k) {
+        if (blob_none(blob, E, k)) continue;
+        blob += E.key_types[k] == TPLX_T_STR ? 4 + blob_u32(blob) : 8;
+    }
+    lens[pos[i]] = blob_none(blob, E, kc) ? 0 : blob_u32(blob);
+}
+// ... and emit key + accumulator columns at the compacted position; a None key gets the placeholder value (0, empty string)
 __global__ void hash_emit(HashTableDev T, const uint64_t *pos, uint64_t n_out, HashEmit E, HashSel sel) {
     uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i == 0)
@@ -375,6 +405,13 @@ __global__ void hash_emit(HashTableDev T, const uint64_t *pos, uint64_t n_out, H
     const uint64_t o = pos[i];
     const uint8_t *blob = T.heap + (T.keyoff[i] & ((1ull << 40) - 1));
     for (uint32_t k = 0; k < E.n_keys; ++k) {
+        const bool none = blob_none(blob, E, k);
+        if (E.key_none[k]) E.key_none[k][o] = none ? 1 : 0;
+        if (none) {
+            if (E.key_types[k] == TPLX_T_STR) E.key_offsets[k][o] = (uint32_t)E.key_lens_scan[k][o];
+            else E.key_data[k][o] = 0;
+            continue;
+        }
         if (E.key_types[k] == TPLX_T_STR) {
             uint32_t len = blob[0] | (blob[1] << 8) | (blob[2] << 16) | ((uint32_t)blob[3] << 24);
             blob += 4;

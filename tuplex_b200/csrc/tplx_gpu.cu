@@ -113,8 +113,9 @@ extern "C" int32_t tplx_gpu_init(const int32_t *devices, int32_t n) {
         CU(cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &thr));
         CU(cudaFuncSetAttribute(stage_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, d->smem_optin));
         CU(cudaFuncSetAttribute(stage_agg_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, d->smem_optin));
-        CU(cudaFuncSetAttribute(stage_hash_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, d->smem_optin));
-        CU(cudaFuncSetAttribute(stage_hash_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, d->smem_optin));
+        CU(cudaFuncSetAttribute(stage_hash_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, d->smem_optin));
+        CU(cudaFuncSetAttribute(stage_hash_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, d->smem_optin));
+        CU(cudaFuncSetAttribute(stage_hash_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, d->smem_optin));
         CU(cudaFuncSetAttribute(stage_mask_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, d->smem_optin));
         CU(cudaFuncSetAttribute(stage_mask_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, d->smem_optin));
         // extra execution lanes on the same GPU (chain d -> alt -> alt ...): two lanes in all let the latency-bound dense
@@ -552,10 +553,18 @@ extern "C" int32_t tplx_gpu_stage_create(const void *desc, uint64_t desc_bytes, 
         if (in.op == TPLX_OP_LDS) s->has_str = true;
     }
     if (h.hidden_out_cols > h.n_out_cols) return bad("stage descriptor: hidden_out_cols out of range");
+    uint32_t key_companions = 0;  // HASH: bit k = key column k has its companion
     for (uint32_t k = 0; k < h.n_out_cols; ++k) {
         const tplx_outcol &oc = s->out_cols[k];
         if (!oc.null_of) continue;
-        if (h.endpoint != TPLX_EP_MEMORY || oc.type != TPLX_T_BOOL || k < h.n_out_cols - h.hidden_out_cols || oc.null_of > h.n_out_cols - h.hidden_out_cols)
+        if (h.endpoint == TPLX_EP_HASH) {
+            const uint32_t key = oc.null_of - 1u;
+            if (oc.type != TPLX_T_BOOL || k < h.n_out_cols - h.hidden_out_cols || k < h.n_keys || key >= h.n_keys ||
+                key >= (uint32_t)(h.n_out_cols - h.hidden_out_cols) || (key_companions >> key & 1u))
+                return bad("stage descriptor: an `is None` companion of a hash stage must be a hidden bool column of one key column");
+            key_companions |= 1u << key;
+        } else if (h.endpoint != TPLX_EP_MEMORY || oc.type != TPLX_T_BOOL || k < h.n_out_cols - h.hidden_out_cols ||
+                   oc.null_of > h.n_out_cols - h.hidden_out_cols)
             return bad("stage descriptor: an `is None` companion must be a hidden bool column of a visible output column");
     }
     s->hidden = h.hidden_out_cols;
@@ -1097,43 +1106,54 @@ static int32_t stage_run_impl(tplx_stage *s, const tplx_block *b, int64_t first_
 template <typename T>
 static int32_t dalloc(tplx_result *r, T **p, size_t count);
 
+// The block plus one "is None" companion column (TPLX_T_BOOL) per entry of `of`: 1 where column of[j] holds None, expanded from that
+// column's validity bitmap (all zeros where the column has no bitmap: it holds no None). The companions are filled on the copy
+// stream; the new block's `ready` event covers them.
+static int32_t expand_companions(const tplx_block *b, const std::vector<uint32_t> &of, tplx_block **out) {
+    for (uint8_t m : b->mapped)
+        if (m) return fail(TPLX_E_UNSUPPORTED, "stage_run: a stage with Option[T] inputs needs device-resident block columns");
+    Device *d = b->dev;
+    CU(cudaSetDevice(d->id));
+    tplx_block *x = new tplx_block();
+    x->dev = d;
+    x->n_rows = b->n_rows;
+    x->cols = b->cols;
+    x->data_bytes = b->data_bytes;
+    x->valid = b->valid;
+    x->valid.resize(b->cols.size(), nullptr);
+    x->csv_quote = b->csv_quote;
+    if (b->ready) CU(cudaStreamWaitEvent(d->copy_stream, b->ready, 0));
+    const uint64_t n = b->n_rows;
+    for (const uint32_t c : of) {
+        void *buf = nullptr;
+        CU(cudaMallocAsync(&buf, n * 8 + 16, d->copy_stream));
+        x->owned.push_back(buf);
+        const uint32_t *v = c < b->valid.size() ? b->valid[c] : nullptr;
+        if (v && n) valid_expand_kernel<<<(uint32_t)((n + 255) / 256), 256, 0, d->copy_stream>>>(v, n, static_cast<uint64_t *>(buf));
+        else CU(cudaMemsetAsync(buf, 0, n * 8 + 16, d->copy_stream));  // a column without a bitmap holds no None
+        ColIn ci{};
+        ci.type = TPLX_T_BOOL;
+        ci.data = buf;
+        x->cols.push_back(ci);
+        x->data_bytes.push_back(n * 8);
+        x->valid.push_back(nullptr);
+    }
+    CU(cudaGetLastError());
+    CU(cudaEventCreateWithFlags(&x->ready, cudaEventDisableTiming));
+    CU(cudaEventRecord(x->ready, d->copy_stream));
+    *out = x;
+    return TPLX_OK;
+}
+
 // Option[T] columns on the way in and out of a stage (option.cuh): companions of the input columns are expanded from the block's
 // validity bitmaps, companions of the output columns are packed into the result's validity bitmaps.
 extern "C" int32_t tplx_gpu_stage_run(tplx_stage *s, const tplx_block *b, int64_t first_row_no, tplx_result **out) {
     if (!s || !b || !out) return fail(TPLX_E_BADARG, "stage_run: bad arguments");
     tplx_block *x = nullptr;
     if (s->n_companions && b->cols.size() + s->n_companions == s->in_types.size()) {
-        for (uint8_t m : b->mapped)
-            if (m) return fail(TPLX_E_UNSUPPORTED, "stage_run: a stage with Option[T] inputs needs device-resident block columns");
-        Device *d = b->dev;
-        CU(cudaSetDevice(d->id));
-        x = new tplx_block();
-        x->dev = d;
-        x->n_rows = b->n_rows;
-        x->cols = b->cols;
-        x->data_bytes = b->data_bytes;
-        x->valid = b->valid;
-        x->csv_quote = b->csv_quote;
-        if (b->ready) CU(cudaStreamWaitEvent(d->copy_stream, b->ready, 0));
-        const uint64_t n = b->n_rows;
-        for (size_t j = b->cols.size(); j < s->in_types.size(); ++j) {
-            const uint32_t c = (uint32_t)s->in_null_of[j];
-            void *buf = nullptr;
-            CU(cudaMallocAsync(&buf, n * 8 + 16, d->copy_stream));
-            x->owned.push_back(buf);
-            const uint32_t *v = c < b->valid.size() ? b->valid[c] : nullptr;
-            if (v && n) valid_expand_kernel<<<(uint32_t)((n + 255) / 256), 256, 0, d->copy_stream>>>(v, n, static_cast<uint64_t *>(buf));
-            else CU(cudaMemsetAsync(buf, 0, n * 8 + 16, d->copy_stream));  // a column without a bitmap holds no None
-            ColIn ci{};
-            ci.type = TPLX_T_BOOL;
-            ci.data = buf;
-            x->cols.push_back(ci);
-            x->data_bytes.push_back(n * 8);
-            x->valid.push_back(nullptr);
-        }
-        CU(cudaGetLastError());
-        CU(cudaEventCreateWithFlags(&x->ready, cudaEventDisableTiming));
-        CU(cudaEventRecord(x->ready, d->copy_stream));
+        const std::vector<uint32_t> of(s->in_null_of.begin() + b->cols.size(), s->in_null_of.end());
+        int32_t rc = expand_companions(b, of, &x);
+        if (rc) return rc;
     }
     int32_t rc = stage_run_impl(s, x ? x : b, first_row_no, out);
     if (rc) {

@@ -721,20 +721,29 @@ class StageCompiler:
         return self.prog
 
     def finish_hash(self, key_cols: Sequence[Union[int, str]], agg_func, combine_func, init, op_id: int) -> Program:
-        """aggregateByKey / unique (PipelineBuilder.cc:1108-1400)."""
+        """aggregateByKey / unique (PipelineBuilder.cc:1108-1400). An Option[T] key keeps None as a group of its own (the reference's
+        null bucket, PipelineBuilder.cc:1148-1170,1263-1310): its "is None" flag goes out as a hidden bool column behind the keys
+        (descriptor: tplx_outcol.null_of), and the device result carries the key column with a validity bitmap."""
         self.begin_op(op_id)
         kidx = [self.col_index(k) for k in key_cols]
         for i in kidx:
-            if self.row[i].null is not None:
-                raise UnsupportedUDF("Option[T] key column (null bucket) takes the interpreter path")
+            if self.row[i].type == T_NONE:
+                raise UnsupportedUDF("a key column that is None for every row is not a normal-case column")
             if self.row[i].type not in (T_I64, T_STR, T_BOOL):
                 raise UnsupportedUDF("f64 keys are not supported (reference: PipelineBuilder.cc:1175-1177)")
         accs = self._lower_aggregate(agg_func, combine_func, init) if agg_func is not None else []
         self.prog.endpoint = C["TPLX_EP_HASH"]
-        keys = [self.row[i] for i in kidx]
-        slots = self._finish(keys + [v for _, v, _ in accs])
+        keys = [plain(self.row[i]) for i in kidx]
+        comps = [(k, self.row[i].null) for k, i in enumerate(kidx)
+                 if self.row[i].null is not None and not (self.is_const(self.row[i].null) and not self.row[i].null.const)]
+        slots = self._finish(keys + [nv for _, nv in comps] + [v for _, v, _ in accs])
         self.prog.n_keys = len(keys)
         self.prog.out_cols = [(s, v.type) for s, v in zip(slots[: len(keys)], keys)]
+        if comps:
+            self.prog.out_cols += [(s, T_BOOL) for s in slots[len(keys): len(keys) + len(comps)]]
+            self.prog.out_null_of = [0] * len(keys) + [k + 1 for k, _ in comps]
+            self.prog.hidden_out_cols = len(comps)
+            slots = slots[: len(keys)] + slots[len(keys) + len(comps):]
         self.prog.out_names = [self.names[i] for i in kidx]
         self.prog.accs = [ir.Acc(kind, s, bits) for (kind, _, bits), s in zip(accs, slots[len(keys):])]
         return self.prog
