@@ -140,6 +140,9 @@ int32_t tplx_gpu_block_from_partitions(int32_t device, const uint8_t *const *par
 int32_t tplx_gpu_block_rows(const tplx_block *block, uint64_t *n_rows);
 /* Device bytes of every column (values, or string payload + offsets): what a kernel reading the block moves. */
 int32_t tplx_gpu_block_column_bytes(const tplx_block *block, uint64_t *bytes, uint32_t max_cols, uint32_t *n_cols);
+/* Validity words of an Option[T] column of a block, as stored: (n_rows + 31) / 32 words, tail bits included; `nullable` = 0 for a
+ * column without a bitmap (nothing is copied). words may be NULL to ask only for `nullable`. */
+int32_t tplx_gpu_block_fetch_validity(const tplx_block *block, uint32_t col, uint32_t *words, uint32_t *nullable);
 int32_t tplx_gpu_block_free(tplx_block *block);
 
 /* ---- execution -------------------------------------------------------------------------- */
@@ -181,9 +184,15 @@ int32_t tplx_gpu_result_exception_partition(tplx_result *res, uint8_t *buf, uint
  * (fast_csvwriter, core/src/physical/PipelineBuilder.cc:1550-1722; quoteForCSV, runtime/src/Runtime.cc:682-738):
  * bool -> true / false, i64 -> decimal, str quoted iff it holds the quote char, the delimiter, '\n' or '\r'. No header
  * (LocalBackend::writeOutput adds it per file). f64 -> 8 fixed decimals, correctly rounded (ryu d2fixed(8) digits); a value of
- * magnitude >= 2^63 makes the call return TPLX_E_UNSUPPORTED (host formatter). Call with buf == NULL for the size. */
+ * magnitude >= 2^63 makes the call return TPLX_E_UNSUPPORTED (host formatter). Call with buf == NULL for the size.
+ * Refuses Option[T] output columns (TPLX_E_UNSUPPORTED); tplx_gpu_result_csv_nulls writes them. */
 int32_t tplx_gpu_result_csv(tplx_result *res, uint32_t n_cols /* first n_cols output columns, 0 = all */, uint8_t delimiter,
                             uint8_t quotechar, uint8_t *buf, uint64_t buf_bytes, uint64_t *bytes_needed);
+/* K7 with None cells: as tplx_gpu_result_csv, and a None cell of an Option[T] output column is written as `null_value`
+ * (NUL-terminated), quoted once like a string cell (fast_csvwriter: null_value = quote(null_value)). A null value longer than
+ * 128 bytes once quoted returns TPLX_E_UNSUPPORTED. */
+int32_t tplx_gpu_result_csv_nulls(tplx_result *res, uint32_t n_cols, uint8_t delimiter, uint8_t quotechar, const char *null_value,
+                                  uint8_t *buf, uint64_t buf_bytes, uint64_t *bytes_needed);
 int32_t tplx_gpu_result_free(tplx_result *res);
 
 /* ---- hash endpoint (aggregateByKey / unique) ---------------------------------------------- */
@@ -276,6 +285,10 @@ int32_t tplx_gpu_stage_hash_exchange(tplx_stage *stage, int32_t device);
  * that do not (cell-count mismatch, null value in a non-Option column, conversion error): those go to the
  * interpreter path as BADPARSE_STRING_INPUT / NULLERROR rows do in the reference (CSVReader.cc:470-520,583-600). */
 #define TPLX_CSV_SKIP 0xFF /* col_types entry: column is not read (projection pushdown, willBeSerialized = false) */
+/* A col_types entry tplx_type | TPLX_T_OPTION reads an Option[T] column (decodeCells, FlattenedTuple.cc:1259-1300): a cell equal
+ * to a null value is None (placeholder 0 / empty string in the block, validity bit clear in tplx_block's bitmap, block row order),
+ * the row stays in the normal case; a non-null cell decodes as in a T column. An Option column cannot be lazy
+ * (TPLX_E_UNSUPPORTED). */
 typedef struct tplx_csv_buffer tplx_csv_buffer; /* CSV bytes resident on a device */
 typedef struct tplx_csv_result tplx_csv_result;
 typedef struct tplx_csv_desc {

@@ -85,6 +85,7 @@ def lib():
         "tplx_gpu_block_from_partitions": ([i32, P(vp), P(u64), u32, P(ct.c_uint8), u32, P(vp)], i32),
         "tplx_gpu_block_rows": ([vp, P(u64)], i32),
         "tplx_gpu_block_column_bytes": ([vp, P(u64), u32, P(u32)], i32),
+        "tplx_gpu_block_fetch_validity": ([vp, u32, vp, P(u32)], i32),
         "tplx_gpu_block_free": ([vp], i32),
         "tplx_gpu_stage_run": ([vp, vp, i64, P(vp)], i32),
         "tplx_gpu_stage_run_host": ([vp, i32, P(CColumn), u32, u64, i64, P(vp)], i32),
@@ -96,6 +97,7 @@ def lib():
         "tplx_gpu_result_partitions": ([vp, u64, vp, u64, P(u64), P(u64), u32, P(u32)], i32),
         "tplx_gpu_result_exception_partition": ([vp, vp, u64, P(u64)], i32),
         "tplx_gpu_result_csv": ([vp, u32, ct.c_uint8, ct.c_uint8, vp, u64, P(u64)], i32),
+        "tplx_gpu_result_csv_nulls": ([vp, u32, ct.c_uint8, ct.c_uint8, ct.c_char_p, vp, u64, P(u64)], i32),
         "tplx_gpu_result_free": ([vp], i32),
         "tplx_gpu_stage_hash_reserve": ([vp, i32, u64], i32),
         "tplx_gpu_stage_hash_finish": ([vp, i32, P(vp)], i32),
@@ -444,6 +446,18 @@ class Block:
         _check(lib().tplx_gpu_block_rows(h, ct.byref(nr)), "tplx_gpu_block_rows")
         return Block(h, nr.value, device)
 
+    def validity(self, c: int) -> Optional[np.ndarray]:
+        """Validity words of an Option[T] column as the block stores them, tail bits included (tplx_gpu_block_fetch_validity);
+        None for a column without a bitmap."""
+        nullable = ct.c_uint32()
+        _check(lib().tplx_gpu_block_fetch_validity(self._h, c, None, ct.byref(nullable)), "block_fetch_validity")
+        if not nullable.value:
+            return None
+        words = np.zeros((int(self.n_rows) + 31) // 32, dtype=np.uint32)
+        if len(words):
+            _check(lib().tplx_gpu_block_fetch_validity(self._h, c, words.ctypes.data, ct.byref(nullable)), "block_fetch_validity")
+        return words
+
     def free(self):
         if self._h:
             lib().tplx_gpu_block_free(self._h)
@@ -542,18 +556,23 @@ class Result:
         raw = buf.tobytes()
         return [raw[offs[p]:offs[p + 1]] for p in range(nparts.value)]
 
-    def csv_bytes(self, delimiter=",", quotechar='"', n_cols: int = 0) -> Optional[bytes]:
+    def csv_bytes(self, delimiter=",", quotechar='"', n_cols: int = 0, null_value: Optional[str] = None) -> Optional[bytes]:
         """First n_cols (0 = all) output columns as CSV text written on the device (K7); None when an f64 cell has a magnitude
-        >= 2^63 (TPLX_E_UNSUPPORTED: the caller formats on the host)."""
+        >= 2^63 (TPLX_E_UNSUPPORTED: the caller formats on the host). With `null_value` (tplx_gpu_result_csv_nulls) a None cell of
+        an Option[T] column is written as that value, quoted once; without it a result with Option[T] columns returns None."""
+        def call(buf, n, need):
+            if null_value is None:
+                return lib().tplx_gpu_result_csv(self._h, n_cols, ord(delimiter), ord(quotechar), buf, n, ct.byref(need))
+            return lib().tplx_gpu_result_csv_nulls(self._h, n_cols, ord(delimiter), ord(quotechar), null_value.encode(), buf, n,
+                                                   ct.byref(need))
         need = ct.c_uint64()
-        rc = lib().tplx_gpu_result_csv(self._h, n_cols, ord(delimiter), ord(quotechar), None, 0, ct.byref(need))
+        rc = call(None, 0, need)
         if rc == -6:  # TPLX_E_UNSUPPORTED
             return None
         _check(rc, "tplx_gpu_result_csv")
         buf = np.empty(need.value, dtype=np.uint8)
         if need.value:
-            _check(lib().tplx_gpu_result_csv(self._h, n_cols, ord(delimiter), ord(quotechar), buf.ctypes.data, need.value, ct.byref(need)),
-                   "tplx_gpu_result_csv")
+            _check(call(buf.ctypes.data, need.value, need), "tplx_gpu_result_csv")
         return buf.tobytes()
 
     def merge_resolved(self, resolved: "Block", row_nos: Sequence[int], first_row_no: int = 0) -> "Result":

@@ -17,7 +17,7 @@ import numpy as np
 from . import backend
 from .backend import Column
 from .dataset import DataSet, Source
-from .ir import T_BOOL, T_F64, T_I64, T_STR
+from .ir import C, T_BOOL, T_F64, T_I64, T_STR
 
 _DEFAULTS = {
     # key names follow tuplex/core/src/ContextOptions.cc:182-300
@@ -235,7 +235,7 @@ class Context:
         if len(sample) == cs.SAMPLE_BYTES:  # keep whole lines only
             sample = sample[: max(sample.rfind(b"\n"), 0)]
         text = sample.decode("utf-8", "replace")
-        delim = delimiter or (_csv.Sniffer().sniff(text[:65536], delimiters=",;|\t").delimiter if text.strip() else ",")
+        delim = delimiter or _sniff_delimiter(text)
         rows = [[c.decode("utf-8", "replace") for c in cells] for cells, _, _ in cs.iter_rows(sample, ord(delim), ord(quotechar))]
         has_header = header if header is not None else (columns is None and bool(rows) and not _looks_numeric(rows[0]))
         names = rows[0] if (has_header and rows) else None
@@ -249,8 +249,32 @@ class Context:
         for c in range(ncols):
             h = type_hints.get(c, type_hints.get(names[c])) if (c in type_hints or names[c] in type_hints) else None
             if h is not None:
-                types[c] = {int: T_I64, float: T_F64, str: T_STR, bool: T_BOOL}[h]
+                types[c] = _hint_type(h)
         return DataSet(self, cs.CsvSource(arrays, list(names), types, delim, quotechar, bool(has_header), nulls))
+
+
+def _sniff_delimiter(text: str) -> str:
+    """The sample's delimiter; ',' when the sample has none to find (a file of one column, like the 311 zip extract)."""
+    if not text.strip():
+        return ","
+    try:
+        return _csv.Sniffer().sniff(text[:65536], delimiters=",;|\t").delimiter
+    except _csv.Error:
+        return ","
+
+
+def _hint_type(h) -> int:
+    """A csv() type hint: int / float / bool / str, or typing.Optional of one of them (an Option[T] column, T | T_OPTION)."""
+    import typing
+    prim = {int: T_I64, float: T_F64, str: T_STR, bool: T_BOOL}
+    if h in prim:
+        return prim[h]
+    args = typing.get_args(h)
+    if len(args) == 2 and type(None) in args:
+        inner = args[0] if args[1] is type(None) else args[1]
+        if inner in prim:
+            return prim[inner] | C["TPLX_T_OPTION"]
+    raise TypeError(f"csv: unsupported type hint {h!r} (int, float, bool, str or typing.Optional of one of them)")
 
 
 def _looks_numeric(cells) -> bool:

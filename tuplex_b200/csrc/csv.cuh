@@ -18,6 +18,8 @@
 //                        packed); rows that do not fit the normal case (cell count, null in a non-Option column,
 //                        conversion error) become exception entries for the interpreter path, like
 //                        BADPARSE_STRING_INPUT rows in the reference (CSVReader.cc:470-520,583-600).
+//   6. csv_pack_valid    Option[T] columns only: a null cell there is None (step 4 records it in the row's null mask),
+//                        and the validity words of the block follow from the masks in block row order.
 // HBM-bound byte work: coalesced 16-byte loads, no tensor cores. Algorithmic traffic per input byte: read 3x (steps
 // 1,3,4) + string payload read+written once.
 #pragma once
@@ -222,6 +224,26 @@ __global__ void __launch_bounds__(CSV_NT) csv_copy_strings(const CsvCompactParam
                 }
             }
         }
+    }
+}
+
+// Validity words of the Option columns, in block (compacted) row order: one thread per block row reads its data row's null
+// mask (csv_parse_one_row) and each warp ballots one word per column; bits past n_good are zero.
+struct CsvValidParams {
+    uint64_t n_good;
+    uint32_t n_opt;
+    const uint64_t *nullmask;  // [nd], per data row
+    const uint32_t *rowmap;    // [n_good], block row -> data row
+    uint8_t slot[TPLX_MAX_COLS];
+    uint32_t *words[TPLX_MAX_COLS];
+};
+__global__ void __launch_bounds__(CSV_NT) csv_pack_valid(const CsvValidParams P) {
+    const uint64_t pos = (uint64_t)blockIdx.x * CSV_NT + threadIdx.x;
+    const uint64_t m = pos < P.n_good ? P.nullmask[P.rowmap[pos]] : ~0ull;
+    const bool write = (threadIdx.x & 31) == 0 && (pos >> 5) < ((P.n_good + 31) >> 5);
+    for (uint32_t k = 0; k < P.n_opt; ++k) {
+        const uint32_t w = __ballot_sync(0xFFFFFFFFu, !((m >> P.slot[k]) & 1ull));
+        if (write) P.words[k][pos >> 5] = w;
     }
 }
 

@@ -558,6 +558,7 @@ struct CsvParseParams {
     uint64_t *good;                // [nd + 1] 1 = normal-case row (scanned in place)
     uint32_t *code;                // [nd] exception code, 0 = good
     uint32_t *flags;               // [0] != 0: a row did not end where quote parity predicted
+    uint64_t *nullmask;            // [nd] bit k set = output column k (an Option column) is None in this row; null when no column is Option
 };
 
 TPLX_HD uint32_t csv_row_start(const uint8_t *buf, const uint32_t *row_end, uint32_t r) {
@@ -570,15 +571,24 @@ TPLX_HD void csv_parse_one_row(const CsvParseParams &P, uint32_t i) {
     const uint32_t r = P.r0 + i;
     const uint32_t start = csv_row_start(P.buf, P.row_end, r), end = P.row_end[r];
     uint32_t code = 0, ncells = 0;
+    if (P.nullmask) P.nullmask[i] = 0;  // set bit by bit below: a mask held in a register across the row machine spills
     const uint32_t got = csv_row_machine(P.buf, start, P.n, P.delim, P.quote, &ncells, [&](uint32_t c, uint32_t b, uint32_t e, bool esc) {
         if (c >= P.n_file_cols || code) return;
-        const uint32_t kind = P.col_kind[c];
+        uint32_t kind = P.col_kind[c];
         if (kind == CSV_SKIP) return;
         const uint32_t slot = P.col_slot[c];
         if (csv_cell_is_null(P.buf, b, e, esc, P.quote, P.nulls)) {
-            code = TPLX_EC_NULLERROR;  // null in a non-Option column (FlattenedTuple.cc:1266-1279)
+            if (!(kind & TPLX_T_OPTION)) {
+                code = TPLX_EC_NULLERROR;  // null in a non-Option column (FlattenedTuple.cc:1266-1279)
+                return;
+            }
+            // None in an Option column (decodeCells, FlattenedTuple.cc:1259-1300): placeholder 0 / empty string, validity bit clear
+            P.nullmask[i] |= 1ull << slot;
+            P.tmp[slot][i] = 0;
+            if (P.strk[slot] >= 0) P.lens[(size_t)P.strk[slot] * (P.nd + 1) + i] = 0;
             return;
         }
+        kind &= ~TPLX_T_OPTION;
         if (kind == TPLX_T_STR) {
             P.tmp[slot][i] = (uint64_t)b | ((uint64_t)(e - b) << 32) | ((uint64_t)esc << 63);
             if (P.strk[slot] >= 0)  // lazy columns (strk < 0) keep the reference only
@@ -618,7 +628,8 @@ TPLX_HD uint32_t csv_find_rows_sequential(const uint8_t *buf, uint32_t n, uint8_
 // ---- CSV sink (K7): one output row as text --------------------------------------------------------------
 // fast_csvwriter (core/src/physical/PipelineBuilder.cc:1550-1722): bool -> true / false, i64 -> decimal (i64toa),
 // str -> quoteForCSV (runtime/src/Runtime.cc:682-738: quoted iff the cell holds a quote, the separator, '\n' or '\r';
-// quotes doubled), cells joined by the delimiter, '\n' after the row. f64 (ryu d2fixed, 8 digits) is not written on
+// quotes doubled), a None cell of an Option column -> the null value quoted once (`null_value = quote(null_value)`),
+// cells joined by the delimiter, '\n' after the row. f64 (ryu d2fixed, 8 digits) is not written on
 // device for |v| < 2^63 (exact integer arithmetic below); larger magnitudes make the call report TPLX_E_UNSUPPORTED and the
 // caller formats on the host.
 TPLX_HD uint32_t csv_i64_len(int64_t v) {
@@ -730,6 +741,8 @@ TPLX_HD uint32_t csv_f64_fixed8(double v, uint8_t *out /* may be null: length on
     return o + nd + 9;
 }
 
+constexpr uint32_t CSV_NULL_CAP = 128;  // bytes of the quoted null value a None cell is written as
+
 struct CsvSinkCols {
     uint32_t n_cols;
     uint8_t delim, quote;
@@ -737,12 +750,20 @@ struct CsvSinkCols {
     const uint64_t *data[TPLX_MAX_COLS];
     const uint32_t *offsets[TPLX_MAX_COLS];
     const uint8_t *bytes[TPLX_MAX_COLS];
+    const uint32_t *valid[TPLX_MAX_COLS];  // Option column: validity words (a clear bit = None cell), else null
+    uint32_t null_len;                     // a None cell is written as null_text[0, null_len): the null value, quoted once
+    uint8_t null_text[CSV_NULL_CAP];
 };
+TPLX_HD bool csv_sink_is_none(const CsvSinkCols &C, uint32_t c, uint64_t r) {
+    return C.valid[c] && !((C.valid[c][r >> 5] >> (r & 31)) & 1u);
+}
 // returns 0 when a cell cannot be formatted here (f64 of magnitude >= 2^63)
 TPLX_HD uint64_t csv_sink_row_len(const CsvSinkCols &C, uint64_t r) {
     uint64_t n = C.n_cols;  // delimiters + newline
     for (uint32_t c = 0; c < C.n_cols; ++c) {
-        if (C.types[c] == TPLX_T_F64) {
+        if (csv_sink_is_none(C, c, r))
+            n += C.null_len;
+        else if (C.types[c] == TPLX_T_F64) {
             const uint32_t l = csv_f64_fixed8(*reinterpret_cast<const double *>(&C.data[c][r]), nullptr);
             if (!l) return 0;
             n += l;
@@ -757,7 +778,9 @@ TPLX_HD uint64_t csv_sink_row_len(const CsvSinkCols &C, uint64_t r) {
 }
 TPLX_HD void csv_sink_row_write(const CsvSinkCols &C, uint64_t r, uint8_t *p) {
     for (uint32_t c = 0; c < C.n_cols; ++c) {
-        if (C.types[c] == TPLX_T_STR)
+        if (csv_sink_is_none(C, c, r)) {
+            for (uint32_t k = 0; k < C.null_len; ++k) *p++ = C.null_text[k];
+        } else if (C.types[c] == TPLX_T_STR)
             p += csv_quoted_write(p, C.bytes[c] + C.offsets[c][r], C.offsets[c][r + 1] - C.offsets[c][r], C.delim, C.quote);
         else if (C.types[c] == TPLX_T_F64)
             p += csv_f64_fixed8(*reinterpret_cast<const double *>(&C.data[c][r]), p);

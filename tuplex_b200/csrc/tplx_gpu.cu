@@ -971,6 +971,18 @@ extern "C" int32_t tplx_gpu_block_column_bytes(const tplx_block *b, uint64_t *by
     return TPLX_OK;
 }
 
+extern "C" int32_t tplx_gpu_block_fetch_validity(const tplx_block *b, uint32_t col, uint32_t *words, uint32_t *nullable) {
+    if (!b || !nullable || col >= b->cols.size()) return fail(TPLX_E_BADARG, "block_fetch_validity: bad arguments");
+    const uint32_t *v = col < b->valid.size() ? b->valid[col] : nullptr;
+    *nullable = v ? 1u : 0u;
+    const uint64_t n_words = (b->n_rows + 31) / 32;
+    if (!v || !words || !n_words) return TPLX_OK;
+    CU(cudaSetDevice(b->dev->id));
+    if (b->ready) CU(cudaEventSynchronize(b->ready));
+    CU(cudaMemcpy(words, v, n_words * 4, cudaMemcpyDeviceToHost));
+    return TPLX_OK;
+}
+
 extern "C" int32_t tplx_gpu_block_free(tplx_block *b) {
     if (!b) return TPLX_OK;
     cudaSetDevice(b->dev->id);

@@ -15,6 +15,7 @@ from __future__ import annotations
 
 import json
 from collections import Counter
+from fractions import Fraction
 from typing import Any, List, Optional, Sequence
 
 import numpy as np
@@ -22,7 +23,9 @@ import numpy as np
 from . import backend
 from .backend import Column
 from .dataset import Source
-from .ir import T_BOOL, T_F64, T_I64, T_STR
+from .ir import C, T_BOOL, T_F64, T_I64, T_STR
+
+T_OPTION = C["TPLX_T_OPTION"]  # type flag of an Option[T] column (col_types of the device CSV source)
 
 SAMPLE_BYTES = 1 << 20
 MAX_CHUNK = 0xFFFFFFFF - (1 << 20)  # tplx_gpu_csv_upload takes < 4 GiB
@@ -203,10 +206,14 @@ def parse_general(s: str, nulls) -> Any:
     return s
 
 
-def decode_typed(cells: Sequence[bytes], types: Sequence[int]) -> tuple:
+def decode_typed(cells: Sequence[bytes], types: Sequence[int], option_cols=(), nulls=()) -> tuple:
+    """Cells as the device decodes them; a null cell of an Option column is None. None also marks a cell that does not convert."""
     out = []
-    for c, t in zip(cells, types):
+    for k, (c, t) in enumerate(zip(cells, types)):
         s = _text(c)
+        if k in option_cols and s in nulls:
+            out.append(None)
+            continue
         out.append(s if t == T_STR else atoi64(s) if t == T_I64 else atod(s) if t == T_F64 else atob(s))
     return tuple(out)
 
@@ -222,21 +229,29 @@ def _cell_kind(s: str) -> int:
 
 
 def infer_types(rows: List[List[str]], ncols: int, nulls, threshold: float = 0.9) -> List[int]:
-    """Majority type per column over the sample; mixed int/float columns become f64 (CSVStatistic's normal case)."""
+    """Majority type per column over the sample; mixed int/float columns become f64 (CSVStatistic's normal case). A column
+    whose null fraction over the sample's data rows exceeds 1 - threshold is Option[T] (T | T_OPTION), and Option[str] when
+    every cell is null (CSVStatistic::estimate with disableNullColumns, utils/src/CSVStatistic.cc:109-140). The comparison is
+    exact, so a column with at most 10 % nulls at threshold 0.9 keeps T."""
     types = []
+    band = 1 - Fraction(str(threshold))
     for c in range(ncols):
-        cnt = Counter(_cell_kind(r[c]) for r in rows if len(r) == ncols and r[c] not in nulls)
+        cells = [r[c] for r in rows if len(r) == ncols]
+        cnt = Counter(_cell_kind(s) for s in cells if s not in nulls)
         tot = sum(cnt.values())
         if not tot:
-            types.append(T_STR)
+            t = T_STR
         elif cnt.get(T_I64, 0) >= threshold * tot:
-            types.append(T_I64)
+            t = T_I64
         elif cnt.get(T_I64, 0) + cnt.get(T_F64, 0) >= threshold * tot:
-            types.append(T_F64)
+            t = T_F64
         elif cnt.get(T_BOOL, 0) >= threshold * tot:
-            types.append(T_BOOL)
+            t = T_BOOL
         else:
-            types.append(T_STR)
+            t = T_STR
+        if cells and Fraction(len(cells) - tot, len(cells)) > band:
+            t |= T_OPTION
+        types.append(t)
     return types
 
 
@@ -251,14 +266,21 @@ class CsvChunk:
 
 
 class CsvSource(Source):
-    """Lazy CSV input: `files` = uint8 arrays (one per file, header row still inside when `header`)."""
+    """Lazy CSV input: `files` = uint8 arrays (one per file, header row still inside when `header`). `types` may carry T_OPTION:
+    such a column is Option[T], its null cells are None in the normal case."""
 
     def __init__(self, files: List[np.ndarray], names: List[Optional[str]], types: List[int], delimiter: str, quotechar: str,
                  header: bool, null_values: Sequence[str]):
-        super().__init__([_TypeOnly(t) for t in types], names, 0, None, [], 0)
-        self.files, self.types = files, list(types)
+        base = [t & ~T_OPTION for t in types]
+        super().__init__([_TypeOnly(t) for t in base], names, 0, None, [], 0)
+        self.files, self.types = files, base
+        self._option_cols = [c for c, t in enumerate(types) if t & T_OPTION]
         self.delimiter, self.quotechar, self.header = delimiter, quotechar, header
         self.null_values = list(null_values)
+
+    @property
+    def option_cols(self) -> List[int]:
+        return self._option_cols
 
     # -- chunks of at most MAX_CHUNK bytes, cut at a newline outside quotes (quote parity, like the device) ----------
     def chunks(self):
@@ -289,16 +311,23 @@ class CsvSource(Source):
 
     def line_object(self, line: bytes, typed: bool):
         """Python value of one row for the interpreter path: typed=True for rows that parsed on the device (values as
-        the device decoded them), False for rows that did not (every cell through `parse`)."""
+        the device decoded them, None for the null cells of Option columns), False for rows that did not (every cell
+        through `parse`)."""
         cells = split_line(line, ord(self.delimiter), ord(self.quotechar))
         if typed and len(cells) == len(self.types):
-            vals = decode_typed(cells, self.types)
+            vals = decode_typed(cells, self.types, self.option_cols, self.null_values)
         else:
             vals = tuple(parse_general(_text(c), self.null_values) for c in cells)
         return vals if len(vals) != 1 else vals[0]
 
+    def _normal_case(self, cells, vals) -> bool:
+        """Does a decoded row fit the normal case: every null cell in an Option column, every other cell converted."""
+        return all((k in self.option_cols) if _text(c) in self.null_values else v is not None
+                   for k, (c, v) in enumerate(zip(cells, vals)))
+
     def to_host_source(self) -> Source:
-        """Whole input through the interpreter-path decoders (used when a stage's UDFs are outside the GPU op set)."""
+        """Whole input through the interpreter-path decoders (used when a stage's UDFs are outside the GPU op set). Null cells
+        of Option columns stay in the normal case as None (validity bitmaps)."""
         normal: List[list] = [[] for _ in self.types]
         orig, fallback = [], []
         i = 0
@@ -308,8 +337,8 @@ class CsvSource(Source):
             for k, (cells, ls, le) in enumerate(iter_rows(raw, d, q)):
                 if skip and k == 0:
                     continue
-                vals = decode_typed(cells, self.types) if len(cells) == len(self.types) else None
-                if vals is None or any(v is None for v in vals) or any(_text(c) in self.null_values for c in cells):
+                vals = decode_typed(cells, self.types, self.option_cols, self.null_values) if len(cells) == len(self.types) else None
+                if vals is None or not self._normal_case(cells, vals):
                     fallback.append((i, self.line_object(raw[ls:le], False)))
                 else:
                     for c, v in enumerate(vals):

@@ -51,6 +51,10 @@ class Source:
         self.fallback = fallback      # (original position, python object)
         self.total_rows = total_rows
 
+    @property
+    def option_cols(self) -> List[int]:
+        return _option_cols(self.cols)
+
 
 class JoinSpec:
     """A JoinOperator of the logical plan (tuplex/core/src/logical/JoinOperator.cc): two upstream datasets, the key column on each
@@ -206,11 +210,11 @@ class DataSet:
 
     def tocsv(self, path, part_size=0, num_rows=None, num_parts=0, part_name_generator=None, null_value=None, header=True):
         """CSV sink (python/tuplex/dataset.py:502-560). Rows are formatted like the reference's row writer
-        (fast_csvwriter, PipelineBuilder.cc:1550-1722): on the device (K7, tplx_gpu_result_csv) when the last stage ran
-        there without rows from the interpreter path, else by the host twin `_csv_cell`."""
+        (fast_csvwriter, PipelineBuilder.cc:1550-1722): on the device (K7, tplx_gpu_result_csv_nulls, None cells as `null_value`)
+        when the last stage ran there without rows from the interpreter path, else by the host twin `_csv_cell`."""
         import os
         chunks: List[bytes] = []
-        rows, names = self._execute(csv_sink=chunks)
+        rows, names = self._execute(csv_sink=chunks, csv_null=null_value or "")
         os.makedirs(path, exist_ok=True) if not path.endswith(".csv") else None
         fn = path if path.endswith(".csv") else os.path.join(path, "part0.csv")
         with open(fn, "wb") as fp:
@@ -297,9 +301,9 @@ class DataSet:
                 pass
         return _map_output_names(op.udf, names)
 
-    def _execute(self, csv_sink: Optional[list] = None):
+    def _execute(self, csv_sink: Optional[list] = None, csv_null: str = ""):
         """Split the operator chain into stages and run them. Returns (python rows, column names). With `csv_sink` (a list) the
-        last stage may instead write its rows there as CSV text and return (None, column names)."""
+        last stage may instead write its rows there as CSV text, None cells as `csv_null`, and return (None, column names)."""
         src = self._source
         self._last_exceptions = Counter()
         if self._join is not None:
@@ -322,7 +326,7 @@ class DataSet:
             if si > 0:
                 src = self._ctx._source_from_rows(rows, names)
             last = si == len(stages) - 1
-            rows, names = _run_stage(self._ctx, src, ops, self._last_exceptions, csv_sink=csv_sink if last else None)
+            rows, names = _run_stage(self._ctx, src, ops, self._last_exceptions, csv_sink=csv_sink if last else None, csv_null=csv_null)
         return rows, names
 
 
@@ -344,10 +348,11 @@ def _map_output_names(udf, names):
     return [None]
 
 
-def csv_lazy_columns(prog, used_cols, in_types):
+def csv_lazy_columns(prog, used_cols, in_types, option_cols=()):
     """File columns the device CSV source may leave as cell references: string columns of a row stage that its prefilter
-    does not read (the stage materialises them for surviving rows only). `prog` reads the projected block `used_cols`."""
-    if prog.prefilter is None or prog.endpoint != C["TPLX_EP_MEMORY"]:
+    does not read (the stage materialises them for surviving rows only). `prog` reads the projected block `used_cols`. None for
+    a stage that reads an Option column: its companions are expanded from a block of device-resident columns."""
+    if prog.prefilter is None or prog.endpoint != C["TPLX_EP_MEMORY"] or any(c in option_cols for c in used_cols):
         return None
     early = {int(i.imm) for i in prog.prefilter.instrs if i.op == C["TPLX_OP_LDCOL"]}
     lazy = [c for k, c in enumerate(used_cols) if k not in early and in_types[c] == T_STR]
@@ -386,7 +391,7 @@ def _option_cols(cols) -> List[int]:
 def _compile_row_ops(src: Source, ops: Sequence[Op]) -> StageCompiler:
     """A stage compiler over `src`'s columns fed the row operators `ops`; UnsupportedUDF for a UDF outside the GPU op set and
     for any operator that is not a row operator."""
-    sc = StageCompiler([c.type for c in src.cols], src.names, _option_cols(src.cols))
+    sc = StageCompiler([c.type for c in src.cols], src.names, src.option_cols)
     for op in ops:
         if op.kind == "map":
             sc.add_map(op.udf, op.id)
@@ -596,7 +601,7 @@ def _py_join_pairs(L, li, R, ri, left_outer, build_right, n_right_cols):
     return out
 
 
-def _run_stage(ctx, src: Source, ops: List[Op], exc_counter: Counter, csv_sink: Optional[list] = None):
+def _run_stage(ctx, src: Source, ops: List[Op], exc_counter: Counter, csv_sink: Optional[list] = None, csv_null: str = ""):
     """One TransformStage on the GPU + CPython resolve of its exception rows."""
     end = ops[-1] if ops and ops[-1].kind in _ENDPOINTS else None
     row_ops = ops[:-1] if end else ops
@@ -614,7 +619,7 @@ def _run_stage(ctx, src: Source, ops: List[Op], exc_counter: Counter, csv_sink: 
     shards = [_csv_blocks(ctx, plan, stage, src, hold)] if is_csv else _column_blocks(ctx, plan, stage, src, hold)
     st = _stitch(shards, src.fallback)
     if end is None:
-        rows, names = _rows_endpoint(plan, st, src, exc_counter, csv_sink), plan.out_names
+        rows, names = _rows_endpoint(plan, st, src, exc_counter, csv_sink, csv_null), plan.out_names
     elif end.kind == "aggregate":
         rows, names = _aggregate_endpoint(plan, st, src.names, exc_counter)
     else:
@@ -720,8 +725,9 @@ def _csv_blocks(ctx, plan: _StagePlan, stage, src, hold: bool) -> _Shard:
     parse become fallback rows; the rows whose UDF raised are decoded from their text as the device decoded them."""
     sh = _Shard(ctx._device)
     in_types = [c.type for c in src.cols]
-    col_types = [t if c in plan.used_cols else backend.CSV_SKIP for c, t in enumerate(in_types)]
-    lazy = csv_lazy_columns(plan.prog, plan.used_cols, in_types)
+    opt = src.option_cols
+    col_types = [(t | (C["TPLX_T_OPTION"] if c in opt else 0)) if c in plan.used_cols else backend.CSV_SKIP for c, t in enumerate(in_types)]
+    lazy = csv_lazy_columns(plan.prog, plan.used_cols, in_types, opt)
     base = 0
     for data, skip_header in src.chunks():
         buf = backend.CsvBuffer(sh.dev, data)
@@ -814,7 +820,7 @@ def _stitch(shards: List[_Shard], fallback: List[Tuple[int, Any]]) -> _Shard:
     return st
 
 
-def _rows_endpoint(plan: _StagePlan, st: _Shard, src: Source, exc_counter: Counter, csv_sink: Optional[list]):
+def _rows_endpoint(plan: _StagePlan, st: _Shard, src: Source, exc_counter: Counter, csv_sink: Optional[list], csv_null: str = ""):
     """Memory endpoint: the normal-case rows with the rows resolved on the CPython path merged in, in order. With a CSV sink
     the device writes the text into `csv_sink` when it can, and None is returned."""
     prog, row_ops = plan.prog, plan.row_ops
@@ -822,11 +828,13 @@ def _rows_endpoint(plan: _StagePlan, st: _Shard, src: Source, exc_counter: Count
     user_cols = ncols - (1 if plan.need_rowidx else 0)
     excs = st.exceptions()
     if csv_sink is not None:
-        # the device row writer (K7) prints values, not None cells. Exception rows resolved in CPython go back into their slots
+        # the device row writer (K7) prints None cells as `csv_null`. Exception rows resolved in CPython go back into their slots
         # ON THE DEVICE (K9, ResolveTask::executeInOrder), except when they must merge with fallback rows by __rowidx
         chunks = None
-        if not st.fallback and not any(prog.out_null_of) and not (len(excs) and plan.need_rowidx):
-            chunks = _device_merge_csv(st.held, row_ops, src.names, st.inputs, [t for _, t in prog.out_cols[:user_cols]], exc_counter)
+        if not st.fallback and not (len(excs) and plan.need_rowidx):
+            option_outs = {k - 1 for k in prog.out_null_of if k}
+            chunks = _device_merge_csv(st.held, row_ops, src.names, st.inputs, [t for _, t in prog.out_cols[:user_cols]], option_outs,
+                                       csv_null, exc_counter)
         if chunks is not None:
             csv_sink.extend(chunks)
             for res, *_ in st.held:
@@ -996,17 +1004,19 @@ def _fits_type(v, t: int) -> bool:
     return isinstance(v, int) and not isinstance(v, bool) and -(1 << 63) <= v < (1 << 63)
 
 
-def _device_merge_csv(held, row_ops, names, inputs: Dict[int, Any], out_types, exc_counter: Counter) -> Optional[List[bytes]]:
+def _device_merge_csv(held, row_ops, names, inputs: Dict[int, Any], out_types, option_outs, null_value: str,
+                      exc_counter: Counter) -> Optional[List[bytes]]:
     """CSV text of every held block result with its resolved exception rows merged in order on the device
-    (tplx_gpu_result_merge_resolved + tplx_gpu_result_csv). None when a resolved row does not fit the stage's output schema
-    (the host path then merges and formats); exception counts are only taken over on success."""
+    (tplx_gpu_result_merge_resolved + tplx_gpu_result_csv_nulls; None cells of the Option output columns `option_outs` are written
+    as `null_value`). None when a resolved row does not fit the stage's output schema (the host path then merges and formats);
+    exception counts are only taken over on success."""
     ncols = len(out_types)
     chunks: List[bytes] = []
     counts: Counter = Counter()
     for res, lo, _rowmap, frn, dev in held:
         ex = res.exceptions()
         if not len(ex):
-            txt = res.csv_bytes(n_cols=ncols)
+            txt = res.csv_bytes(n_cols=ncols, null_value=null_value)
             if txt is None:
                 return None
             chunks.append(txt)
@@ -1017,13 +1027,13 @@ def _device_merge_csv(held, row_ops, names, inputs: Dict[int, Any], out_types, e
             if r is None:
                 continue
             vt = r[0] if isinstance(r[0], tuple) else (r[0],)
-            if len(vt) != ncols or not all(_fits_type(v, t) for v, t in zip(vt, out_types)):
+            if len(vt) != ncols or not all(_fits_type(v, t) or (v is None and c in option_outs) for c, (v, t) in enumerate(zip(vt, out_types))):
                 return None
             rows.append(vt)
             nos.append(int(e["row_no"]))
         blk = backend.Block.upload(dev, [Column.from_values([r[c] for r in rows], out_types[c]) for c in range(ncols)], len(rows))
         merged = res.merge_resolved(blk, nos, frn)
-        txt = merged.csv_bytes(n_cols=ncols)
+        txt = merged.csv_bytes(n_cols=ncols, null_value=null_value)
         merged.free()
         blk.free()
         if txt is None:

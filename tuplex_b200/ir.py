@@ -171,12 +171,13 @@ def pack_scan_terms(terms: List[dict]) -> bytes:
 
 
 def referenced_inputs(prog: Program) -> List[int]:
-    """Input columns a stage actually loads (projection pushdown: the reference keeps only these when it reads a
-    file, LogicalOptimizer projection pushdown / `columnsToSerialize`, StageBuilder.cc:1045-1070)."""
+    """Physical input columns a stage actually loads (projection pushdown: the reference keeps only these when it reads a
+    file, LogicalOptimizer projection pushdown / `columnsToSerialize`, StageBuilder.cc:1045-1070). A load of an "is None"
+    companion counts as a use of its Option[T] column, whose validity bitmap fills the companion."""
     used = set()
     p = prog
     while p is not None:
-        used.update(int(i.imm) for i in p.instrs if i.op == C["TPLX_OP_LDCOL"])
+        used.update(p.null_of.get(int(i.imm), int(i.imm)) for i in p.instrs if i.op == C["TPLX_OP_LDCOL"])
         p = p.prefilter
     if prog.fused and scan_terms(prog.fused) is None:
         _, n_preds, n_terms, _ = struct.unpack_from("<IIII", prog.fused, 0)
@@ -195,15 +196,21 @@ def referenced_inputs(prog: Program) -> List[int]:
 
 
 def project_inputs(prog: Program, used: List[int]) -> None:
-    """Renumber the input columns of `prog` (in place) so that it reads a block holding only `used`."""
+    """Renumber the input columns of `prog` (in place) so that it reads a block holding only the physical columns `used`. The
+    companion of every projected Option[T] column follows them, in the order of its column, where the executor appends the
+    companions (tplx_gpu_stage_run); companions of columns left out are dropped."""
     remap = {c: k for k, c in enumerate(used)}
     p = prog
     while p is not None:
+        comps = sorted((c, j) for j, c in p.null_of.items() if c in remap)
+        cmap = {j: len(used) + m for m, (_, j) in enumerate(comps)}
         for i in p.instrs:
             if i.op == C["TPLX_OP_LDCOL"]:
-                i.imm = remap[int(i.imm)]
-        p.in_types = [p.in_types[c] for c in used]
-        p.in_names = [p.in_names[c] for c in used] if p.in_names else p.in_names
+                i.imm = cmap[int(i.imm)] if int(i.imm) in p.null_of else remap[int(i.imm)]
+        keep = list(used) + [j for _, j in comps]
+        p.in_types = [p.in_types[c] for c in keep]
+        p.in_names = [p.in_names[c] for c in keep] if p.in_names else p.in_names
+        p.null_of = {cmap[j]: remap[c] for c, j in comps}
         terms = scan_terms(p.fused)
         if terms is not None:  # string-scan hint of a (prefilter) row stage: its terms name input columns too
             for t in terms:
