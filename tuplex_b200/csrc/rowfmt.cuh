@@ -5,7 +5,13 @@
 //   row  = [one 8-byte slot per field][8 B total var-len bytes iff any var-len field][var-len payload]
 //   slot = i64 | f64 bits | bool as i64 | (offset_from_slot_address & 0xFFFFFFFF) | (size_incl_NUL << 32)
 //   partition = int64 numRows, then rows back to back.
-// (The bitmap prefix of Option[] schemas does not occur on the normal-case path handled here.)
+// A schema with Option[T] fields prefixes each row with a bitmap of ceil(n_opt / 64) 8-byte words (Serializer.cc:1041-1059, see
+// RowFmtCols). The reader accepts the three forms a None string field takes in the reference's rows:
+//   "" of size 0, slot = offset | 0              (a None produced by a UDF, FlattenedTuple.cc:628; what write_row writes)
+//   slot = 0 when the row has no var-len bytes   (Serializer.cc:313-338, 1071: slots are filled only when there are bytes)
+//   the null cell's text, slot = offset | size   (the compiled CSV path, FlattenedTuple.cc:1255-1293, 798-835: "N/A\0" in the
+//                                                 payload and in the var-len total)
+// A None field's slot value is never used: it becomes "" (strings) or 0 (numbers) in the column block.
 // Exception record = int64 rowNo, ecCode, opID, size, then the ORIGINAL input row
 // (core/include/physical/IExceptionableTask.h:22-36).
 #pragma once
@@ -148,7 +154,8 @@ __global__ void rows_to_cols_pass1(const uint8_t *__restrict__ rows, const uint6
         else C.data[c][i] = isnull ? 0 : v;
     }
 }
-// pass 2: string bytes (lens now holds exclusive byte offsets)
+// pass 2: string bytes (lens now holds exclusive byte offsets). The length is the one pass 1 counted, never the slot's: a None
+// field may carry the null cell's text in its slot (the compiled CSV path), and pass 1 counted 0 bytes for it.
 __global__ void rows_to_cols_pass2(const uint8_t *__restrict__ rows, const uint64_t *__restrict__ row_off, uint64_t n,
                                    RowFmtCols C, const uint64_t *__restrict__ lens) {
     uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -158,10 +165,10 @@ __global__ void rows_to_cols_pass2(const uint8_t *__restrict__ rows, const uint6
         const uint64_t o = lens[(size_t)C.strk[c] * (n + 1) + i];
         C.offsets[c][i] = (uint32_t)o;
         if (i == n) continue;
+        const uint32_t len = (uint32_t)(lens[(size_t)C.strk[c] * (n + 1) + i + 1] - o);
+        if (!len) continue;  // "" or None: the slot is not read
         const uint8_t *slot = rows + row_off[i] + C.bitmap_bytes + 8 * (size_t)c;
-        const uint64_t v = ld64u(slot);
-        const uint8_t *src = slot + (uint32_t)v;
-        const uint32_t len = (v >> 32) ? (uint32_t)(v >> 32) - 1 : 0;
+        const uint8_t *src = slot + (uint32_t)ld64u(slot);
         uint8_t *dst = C.bytes[c] + o;
         for (uint32_t k = 0; k < len; ++k) dst[k] = src[k];
     }
