@@ -125,8 +125,10 @@ TPLX_HD void str_copy(uint8_t *dst, const StrV &s) {
     for (; i < n; ++i) dst[i] = sch(s, i);
 }
 
+// The out-of-line primitives (here and in vm.cuh) take their views by value: a reference parameter makes every call store the
+// caller's StrV to the thread's stack and the callee load it back, local-memory traffic on every string op of a row function.
 // a == b (both possibly case-flagged)
-TPLX_HD_NOINLINE bool str_eq(const StrV &a, const StrV &b) {
+TPLX_HD_NOINLINE bool str_eq(StrV a, StrV b) {
     if (a.len != b.len) return false;
     WordReader ra, rb;
     ra.init(a);
@@ -217,7 +219,7 @@ TPLX_HD int64_t str_find_impl(const StrV &h, const StrV &n) {
     return -1;
 }
 
-TPLX_HD_NOINLINE int64_t str_find(const StrV &h, const StrV &n) {
+TPLX_HD_NOINLINE int64_t str_find(StrV h, StrV n) {
     if (n.len == 0) return 0;
     if (n.len > h.len) return -1;
     if (h.flags == TPLX_SF_LOWER) return str_find_impl<TPLX_SF_LOWER>(h, n);
@@ -268,7 +270,7 @@ TPLX_HD int64_t str_rfind_impl(const StrV &h, const StrV &n) {
     return -1;
 }
 
-TPLX_HD_NOINLINE int64_t str_rfind(const StrV &h, const StrV &n) {
+TPLX_HD_NOINLINE int64_t str_rfind(StrV h, StrV n) {
     if (n.len > h.len) return -1;
     if (n.len == 0) return (int64_t)h.len;
     if (h.flags == TPLX_SF_LOWER) return str_rfind_impl<TPLX_SF_LOWER>(h, n);

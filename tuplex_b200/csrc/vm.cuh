@@ -47,7 +47,7 @@ struct ColIn {
 };
 
 // float(str): out of line so that the VM's register allocation is not shaped by a rarely used op
-TPLX_HD_NOINLINE bool str_to_f64(const StrV &s, double *out) {
+TPLX_HD_NOINLINE bool str_to_f64(StrV s, double *out) {
     return csv_atod_g([&s](uint32_t k) { return sch(s, k); }, s.len, out);
 }
 
@@ -150,7 +150,7 @@ __device__ __forceinline__ bool op_sconcat(VMThread &t, const StrV &x, const Str
     *out = mk_strv(o, x.len + y.len, 0);
     return true;
 }
-TPLX_OPFN_HEAVY bool op_sreplace(VMThread &t, const StrV &s, const StrV &f, const StrV &r, uint32_t opidx, StrV *out) {
+TPLX_OPFN_HEAVY bool op_sreplace(VMThread &t, StrV s, StrV f, StrV r, uint32_t opidx, StrV *out) {
     // runtime/src/Runtime.cc:401-540
     if (s.len == 0 || (f.len == 0 && r.len == 0)) { *out = s; return true; }
     if (f.len == 0) {
