@@ -332,6 +332,23 @@ int32_t tplx_gpu_csv_result_fetch_rowmap(tplx_csv_result *res, uint32_t *rowmap 
 int32_t tplx_gpu_csv_result_fetch_row_ends(tplx_csv_result *res, uint32_t *ends /* n_rows + 1 */);
 int32_t tplx_gpu_csv_result_free(tplx_csv_result *res);
 
+/* ---- text source (K10) ---------------------------------------------------------------------- */
+/* Replaces the host reader of Context.text (python/tuplex/context.py:367-387) and the reference's TextReader
+ * (core/src/physical/TextReader.cc:60-140; null values: FileInputOperator.cc:144-149) in front of a TransformStage: a buffer
+ * from tplx_gpu_csv_upload becomes a block of one string column, a line per row. Lines end at '\n' (the buffer's appended
+ * newline ends an unterminated last line and nothing else); one trailing '\r' is stripped; a line that is not valid UTF-8 is
+ * stored as CPython's bytes.decode("utf-8", "replace") gives it (one U+FFFD per maximal invalid subpart); a line equal to a
+ * null value after the strip and the replacement is null. With `option`, a null line is None (empty string, validity bit clear
+ * in the block's bitmap); without, it is a bad row (TPLX_EC_NULLERROR) for the interpreter path. The result object is the CSV
+ * source's: info, bad rows, rowmap and row ends (ends[i] + 1 .. ends[i + 1] = line i, newline excluded) are fetched with the
+ * tplx_gpu_csv_result_* calls. A string column above 4 GiB (up to 3x the input after replacement) returns TPLX_E_OVERFLOW. */
+typedef struct tplx_text_desc {
+    uint8_t n_null_values;          /* <= 8, together <= 64 bytes (UTF-8) */
+    uint8_t option;                 /* 1: null lines are None in an Option[str] column; 0: they are bad rows */
+    const char *const *null_values; /* NUL-terminated */
+} tplx_text_desc;
+int32_t tplx_gpu_text_parse(tplx_csv_buffer *buf, const tplx_text_desc *desc, tplx_block **out_block, tplx_csv_result **out_res);
+
 #ifdef __cplusplus
 }
 #endif

@@ -52,6 +52,10 @@ class CCsvInfo(ct.Structure):
                 ("kernel_launches", ct.c_uint32), ("parse_ms", ct.c_double)]
 
 
+class CTextDesc(ct.Structure):
+    _fields_ = [("n_null_values", ct.c_uint8), ("option", ct.c_uint8), ("null_values", ct.POINTER(ct.c_char_p))]
+
+
 CSV_SKIP = 0xFF
 CSV_BAD_DTYPE = np.dtype([("row", "<u4"), ("code", "<u4"), ("line_start", "<u4"), ("line_end", "<u4")])
 EXC_DTYPE = np.dtype([("row", "<i8"), ("row_no", "<i8"), ("code", "<i8"), ("op_id", "<i8")])
@@ -126,6 +130,7 @@ def lib():
         "tplx_gpu_csv_result_fetch_rowmap": ([vp, vp], i32),
         "tplx_gpu_csv_result_fetch_row_ends": ([vp, vp], i32),
         "tplx_gpu_csv_result_free": ([vp], i32),
+        "tplx_gpu_text_parse": ([vp, P(CTextDesc), P(vp), P(vp)], i32),
     }
     for name, (argtypes, restype) in sig.items():
         fn = getattr(L, name)  # AttributeError if the library does not export a declared symbol
@@ -685,6 +690,20 @@ class CsvBuffer:
         nr = ct.c_uint64()
         _check(lib().tplx_gpu_block_rows(hb, ct.byref(nr)), "tplx_gpu_block_rows")
         return CsvParse(Block(hb, nr.value, self.device), hr, [t for t in col_types if t != CSV_SKIP])
+
+    def parse_text(self, null_values: Sequence[str] = (), option: bool = False) -> "CsvParse":
+        """K10 (tplx_gpu_text_parse): every line one row of a single string column. A line equal to a null value is None with
+        `option` (Option[str] column), else a bad row (NULLERROR) for the interpreter path."""
+        d = CTextDesc()
+        d.n_null_values = len(null_values)
+        d.option = int(bool(option))
+        nv = (ct.c_char_p * max(1, len(null_values)))(*[s.encode() for s in null_values])
+        d.null_values = nv
+        hb, hr = ct.c_void_p(), ct.c_void_p()
+        _check(lib().tplx_gpu_text_parse(self._h, ct.byref(d), ct.byref(hb), ct.byref(hr)), "tplx_gpu_text_parse")
+        nr = ct.c_uint64()
+        _check(lib().tplx_gpu_block_rows(hb, ct.byref(nr)), "tplx_gpu_block_rows")
+        return CsvParse(Block(hb, nr.value, self.device), hr, [T_STR])
 
     def free(self):
         if self._h:

@@ -56,6 +56,8 @@ class Metrics:
         self.kernel_launches = 0
         self.csv_rows = self.csv_bad_rows = 0  # rows the device CSV source found / handed to the interpreter path
         self.csv_parse_ms = 0.0
+        self.text_rows = 0  # lines the device text source split
+        self.text_parse_ms = 0.0
 
     def _add(self, info):
         self.rows_in += int(info.n_in_rows)
@@ -202,22 +204,10 @@ class Context:
 
     def text(self, pattern, null_values=None) -> DataSet:
         """tuplex.Context.text (python/tuplex/context.py:367-387): every line of the files is one row of type str; lines equal to a
-        null value become None (the column is then Option[str])."""
-        null_values = list(null_values or [])
-        lines: List[Optional[str]] = []
-        for fn in sorted(f for p in pattern.split(",") for f in (glob.glob(p) or [p])):
-            try:
-                with open(fn, "r", encoding="utf-8", errors="replace", newline="") as fp:
-                    data = fp.read()
-            except OSError:
-                self._log(f"text: no such file {fn!r}")
-                continue
-            part = data.split("\n")
-            if part and part[-1] == "":
-                part.pop()  # the newline that ends the last line does not start another one
-            lines.extend(ln[:-1] if ln.endswith("\r") else ln for ln in part)
-        rows = [None if ln in null_values else ln for ln in lines]
-        return DataSet(self, self._source_from_rows(rows, None))
+        null value become None (the column is then Option[str]). Planning reads the files on the host; the lines themselves are
+        split on the GPU when the first stage runs (textsource.TextSource -> tplx_gpu_text_parse)."""
+        from .textsource import text_source
+        return DataSet(self, text_source(self, pattern, null_values))
 
     def csv(self, pattern, columns=None, header=None, delimiter=None, quotechar='"', null_values=[''], type_hints={}) -> DataSet:
         """tuplex.Context.csv (python/tuplex/context.py:203-290). Planning (delimiter, header, normal-case types) looks at

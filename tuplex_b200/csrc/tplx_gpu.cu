@@ -28,6 +28,7 @@
 #include "mask.cuh"
 #include "vecvm.cuh"
 #include "csv.cuh"
+#include "text.cuh"
 #include "join.cuh"
 #include "option.cuh"
 #include "merge.cuh"
@@ -2329,6 +2330,7 @@ extern "C" int32_t tplx_gpu_result_fetch_aggregate(tplx_result *r, int64_t *acc_
 #include "tplx_gpu_rowfmt.inl"
 #include "tplx_gpu_hash.inl"
 #include "tplx_gpu_csv.inl"
+#include "tplx_gpu_text.inl"
 #include "tplx_gpu_comm.inl"
 #include "tplx_gpu_join.inl"
 #include "tplx_gpu_merge.inl"

@@ -22,7 +22,7 @@ import numpy as np
 
 from . import backend
 from .backend import Column
-from .dataset import Source
+from .dataset import FileSource, Source, csv_lazy_columns
 from .ir import C, T_BOOL, T_F64, T_I64, T_STR
 
 T_OPTION = C["TPLX_T_OPTION"]  # type flag of an Option[T] column (col_types of the device CSV source)
@@ -265,9 +265,11 @@ class CsvChunk:
         self.data, self.skip_header, self.base = data, skip_header, base
 
 
-class CsvSource(Source):
+class CsvSource(FileSource):
     """Lazy CSV input: `files` = uint8 arrays (one per file, header row still inside when `header`). `types` may carry T_OPTION:
     such a column is Option[T], its null cells are None in the normal case."""
+
+    projects = True
 
     def __init__(self, files: List[np.ndarray], names: List[Optional[str]], types: List[int], delimiter: str, quotechar: str,
                  header: bool, null_values: Sequence[str]):
@@ -308,6 +310,30 @@ class CsvSource(Source):
                 lo = hi
                 if n == 0:
                     break
+
+    def cost(self) -> int:
+        """Data rows = line ends of the files (the reference estimates from a sample)."""
+        return int(sum(int(np.count_nonzero(a == 10)) for a in self.files))
+
+    def parse(self, buf, skip_header: bool, plan):
+        """K6 over one chunk: only the file columns the stage's program loads are decoded (projection pushdown)."""
+        opt = self.option_cols
+        col_types = [(t | (T_OPTION if c in opt else 0)) if c in plan.used_cols else backend.CSV_SKIP for c, t in enumerate(self.types)]
+        lazy = csv_lazy_columns(plan.prog, plan.used_cols, self.types, opt)
+        return buf.parse(col_types, self.delimiter, self.quotechar, skip_header, self.null_values, lazy=lazy)
+
+    def count(self, metrics, info):
+        metrics.csv_rows += int(info.n_rows)
+        metrics.csv_bad_rows += int(info.n_bad)
+        metrics.csv_parse_ms += float(info.parse_ms)
+
+    def bad_row_object(self, raw: bytes, bad):
+        return self.line_object(raw[int(bad["line_start"]):int(bad["line_end"])], False)
+
+    def row_object(self, raw: bytes, start: int, end: int):
+        while raw[start] in (10, 13):  # newlines between rows belong to no row
+            start += 1
+        return self.line_object(raw[start:end], True)
 
     def line_object(self, line: bytes, typed: bool):
         """Python value of one row for the interpreter path: typed=True for rows that parsed on the device (values as

@@ -55,6 +55,42 @@ class Source:
     def option_cols(self) -> List[int]:
         return _option_cols(self.cols)
 
+    def cost(self) -> int:
+        return int(self.total_rows)
+
+
+class FileSource(Source):
+    """Input of a plan that is raw file bytes, parsed on one device right in front of the first stage: CSV (K6,
+    csvsource.CsvSource) and text (K10, textsource.TextSource). Planning (names, types, Option columns, cost) is done on the host
+    without a device; rows that the device parse hands back (bad rows) become fallback rows of the stage."""
+
+    plan_types = False  # DataSet.types may come from the plan alone (else from the first rows)
+    projects = False    # the parse decodes only the file columns a stage loads (_StagePlan.used_cols)
+
+    def chunks(self):
+        """(uint8 array, argument of `parse`) per device buffer, in row order."""
+        raise NotImplementedError
+
+    def parse(self, buf, arg, plan):
+        """The chunk resident in `buf` (backend.CsvBuffer) parsed for `plan`'s program: a backend.CsvParse."""
+        raise NotImplementedError
+
+    def count(self, metrics, info):
+        """Add one parse's counters to ctx.metrics."""
+        raise NotImplementedError
+
+    def bad_row_object(self, raw: bytes, bad):
+        """Python object of a bad row (tplx_csv_bad_row `bad` of the chunk text `raw`) for the interpreter path."""
+        raise NotImplementedError
+
+    def row_object(self, raw: bytes, start: int, end: int):
+        """Python object of the row in raw[start:end] as the device parsed it (for rows whose UDF raised on the device)."""
+        raise NotImplementedError
+
+    def to_host_source(self) -> Source:
+        """The whole input as a host Source (stages whose UDFs are outside the GPU op set)."""
+        raise NotImplementedError
+
 
 class JoinSpec:
     """A JoinOperator of the logical plan (tuplex/core/src/logical/JoinOperator.cc): two upstream datasets, the key column on each
@@ -137,9 +173,7 @@ class DataSet:
         src = self._source
         if src is None:
             return 0
-        if hasattr(src, "chunks"):  # CSV source: data rows = line ends of the files (the reference estimates from a sample)
-            return int(sum(int(np.count_nonzero(a == 10)) for a in getattr(src, "files", [])))
-        return int(src.total_rows)
+        return src.cost()
 
     def map(self, ftor):
         return self._with(Op("map", ftor))
@@ -240,7 +274,8 @@ class DataSet:
         typed from their first rows."""
         import typing
         py = {T_I64: int, T_F64: float, T_BOOL: bool, T_STR: str}
-        if self._join is None and self._parent is None and self._source is not None and not hasattr(self._source, "chunks"):
+        src = self._source
+        if self._join is None and self._parent is None and src is not None and (not isinstance(src, FileSource) or src.plan_types):
             try:
                 sc = _compile_row_ops(self._source, self._ops)
                 return [typing.Optional[py[v.type]] if v.null is not None else py[v.type] for v in sc.row]
@@ -605,18 +640,18 @@ def _run_stage(ctx, src: Source, ops: List[Op], exc_counter: Counter, csv_sink: 
     """One TransformStage on the GPU + CPython resolve of its exception rows."""
     end = ops[-1] if ops and ops[-1].kind in _ENDPOINTS else None
     row_ops = ops[:-1] if end else ops
-    is_csv = hasattr(src, "chunks")  # csvsource.CsvSource: the device parses the file right in front of the stage
-    if is_csv and not src.cols:  # missing / empty file: nothing to run (python/tests/test_csv.py:66-69)
+    is_file = isinstance(src, FileSource)  # the device parses the file right in front of the stage
+    if is_file and not src.cols:  # missing / empty file: nothing to run (python/tests/test_csv.py:66-69)
         return _run_stage_python(Source([], [], 0, None, [], 0), ops, exc_counter)
     try:
         plan = _compile_stage(src, row_ops, end)
     except UnsupportedUDF as e:
         ctx._log(f"stage falls back to the CPython path: {e}")
-        return _run_stage_python(src.to_host_source() if is_csv else src, ops, exc_counter)
+        return _run_stage_python(src.to_host_source() if is_file else src, ops, exc_counter)
     backend.init(sorted(set(ctx._devices)))
     stage = backend.Stage(plan.prog)
     hold = csv_sink is not None
-    shards = [_csv_blocks(ctx, plan, stage, src, hold)] if is_csv else _column_blocks(ctx, plan, stage, src, hold)
+    shards = [_file_blocks(ctx, plan, stage, src, hold)] if is_file else _column_blocks(ctx, plan, stage, src, hold)
     st = _stitch(shards, src.fallback)
     if end is None:
         rows, names = _rows_endpoint(plan, st, src, exc_counter, csv_sink, csv_null), plan.out_names
@@ -650,12 +685,12 @@ class _StagePlan:
 
 def _compile_stage(src: Source, row_ops: List[Op], end: Optional[Op]) -> _StagePlan:
     """The stage's device program; UnsupportedUDF when it has to run on the CPython path. A row stage over input that has rows
-    the device does not run (fallback rows, bad CSV rows) also outputs the input row number of each row (__rowidx), by which
-    those rows are merged back in. A CSV stage decodes only the file columns the program loads (projection pushdown)."""
-    is_csv = hasattr(src, "chunks")
+    the device does not run (fallback rows, bad rows of a file source) also outputs the input row number of each row (__rowidx), by
+    which those rows are merged back in. A CSV stage decodes only the file columns the program loads (projection pushdown)."""
+    projects = isinstance(src, FileSource) and src.projects
     sc = _compile_row_ops(src, row_ops)
     out_names = list(sc.names)
-    need_rowidx = end is None and (bool(src.fallback) or is_csv)
+    need_rowidx = end is None and (bool(src.fallback) or isinstance(src, FileSource))
     if end is None:
         if need_rowidx:
             sc.begin_op(row_ops[-1].id if row_ops else 0)
@@ -671,7 +706,7 @@ def _compile_stage(src: Source, row_ops: List[Op], end: Optional[Op]) -> _StageP
     else:
         prog = sc.finish_hash(list(range(len(sc.row))), None, None, None, end.id)
     used_cols = None
-    if is_csv:
+    if projects:
         used_cols = ir.referenced_inputs(prog)
         if len(used_cols) > C["TPLX_MAX_COLS"]:
             raise UnsupportedUDF(f"stage reads {len(used_cols)} columns (> TPLX_MAX_COLS)")
@@ -720,38 +755,29 @@ class _Shard:
         return [self.inputs[int(e["row"])] for e in self.exceptions()] + [obj for _, obj in self.fallback]
 
 
-def _csv_blocks(ctx, plan: _StagePlan, stage, src, hold: bool) -> _Shard:
-    """The block loop of a CSV source: one device parses chunk after chunk (K6) right in front of the stage. Rows that do not
-    parse become fallback rows; the rows whose UDF raised are decoded from their text as the device decoded them."""
+def _file_blocks(ctx, plan: _StagePlan, stage, src: FileSource, hold: bool) -> _Shard:
+    """The block loop of a file source: one device parses chunk after chunk (K6 / K10) right in front of the stage. Bad rows
+    become fallback rows; the rows whose UDF raised are decoded from their text as the device decoded them."""
     sh = _Shard(ctx._device)
-    in_types = [c.type for c in src.cols]
-    opt = src.option_cols
-    col_types = [(t | (C["TPLX_T_OPTION"] if c in opt else 0)) if c in plan.used_cols else backend.CSV_SKIP for c, t in enumerate(in_types)]
-    lazy = csv_lazy_columns(plan.prog, plan.used_cols, in_types, opt)
     base = 0
-    for data, skip_header in src.chunks():
+    for data, arg in src.chunks():
         buf = backend.CsvBuffer(sh.dev, data)
-        parse = buf.parse(col_types, src.delimiter, src.quotechar, skip_header, src.null_values, lazy=lazy)
+        parse = src.parse(buf, arg, plan)
         res = stage.run(parse.block, sh.row_no)
         pinfo, exc, rowmap = parse.info, res.exceptions(), None
-        ctx.metrics.csv_rows += int(pinfo.n_rows)
-        ctx.metrics.csv_bad_rows += int(pinfo.n_bad)
-        ctx.metrics.csv_parse_ms += float(pinfo.parse_ms)
+        src.count(ctx.metrics, pinfo)
         raw = data.tobytes() if (pinfo.n_bad or len(exc)) else b""
         if pinfo.n_bad:  # block row -> data row
             rowmap = parse.rowmap().astype(np.int64)
             for bad in parse.bad_rows():
-                sh.fallback.append((base + int(bad["row"]), src.line_object(raw[int(bad["line_start"]):int(bad["line_end"])], False)))
+                sh.fallback.append((base + int(bad["row"]), src.bad_row_object(raw, bad)))
         if len(exc):
             if rowmap is not None:
                 exc["row"] = rowmap[exc["row"]]
             ends = parse.row_ends().astype(np.int64)
             ends[0] = -1 if ends[0] == 0xFFFFFFFF else ends[0]
             for r in exc["row"]:
-                a = int(ends[r]) + 1
-                while raw[a] in (10, 13):
-                    a += 1
-                sh.inputs[base + int(r)] = src.line_object(raw[a:int(ends[r + 1])], True)
+                sh.inputs[base + int(r)] = src.row_object(raw, int(ends[r]) + 1, int(ends[r + 1]))
         sh.take(ctx, plan, res, base, exc, rowmap, hold)
         base += int(pinfo.n_rows)
         parse.free()
