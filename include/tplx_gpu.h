@@ -144,6 +144,14 @@ int32_t tplx_gpu_block_column_bytes(const tplx_block *block, uint64_t *bytes, ui
  * column without a bitmap (nothing is copied). words may be NULL to ask only for `nullable`. */
 int32_t tplx_gpu_block_fetch_validity(const tplx_block *block, uint32_t col, uint32_t *words, uint32_t *nullable);
 int32_t tplx_gpu_block_free(tplx_block *block);
+/* The rows of n_parts blocks, in order, as one new block on the parts' device that owns its memory (e.g. the build side of a
+ * join whose stage produced several block results). Fixed-width columns and string bytes are copied; string offsets are rebased by
+ * each part's byte position and validity words realigned to each part's first row, one batched launch per column. A column gets a
+ * bitmap when any part has one (a part without one contributes set bits); bits past a part's row count are ignored and the
+ * output's tail bits are zero. String buffers are 4-byte-multiple allocations readable up to the next 16-byte boundary. Parts on
+ * different devices or with different column counts / types: TPLX_E_BADARG; a string column above 4 GiB: TPLX_E_OVERFLOW. Zero
+ * parts give an empty block with no columns on the first initialised device. The parts may be freed when the call returns. */
+int32_t tplx_gpu_block_concat(const tplx_block *const *parts, uint32_t n_parts, tplx_block **out);
 
 /* ---- execution -------------------------------------------------------------------------- */
 /* Run the stage over one block (asynchronously on the device's stream; results are complete

@@ -91,6 +91,7 @@ def lib():
         "tplx_gpu_block_column_bytes": ([vp, P(u64), u32, P(u32)], i32),
         "tplx_gpu_block_fetch_validity": ([vp, u32, vp, P(u32)], i32),
         "tplx_gpu_block_free": ([vp], i32),
+        "tplx_gpu_block_concat": ([P(vp), u32, P(vp)], i32),
         "tplx_gpu_stage_run": ([vp, vp, i64, P(vp)], i32),
         "tplx_gpu_stage_run_host": ([vp, i32, P(CColumn), u32, u64, i64, P(vp)], i32),
         "tplx_gpu_result_info": ([vp, P(CResultInfo)], i32),
@@ -374,6 +375,7 @@ class Stage:
                "tplx_gpu_stage_run_host")
         r = Result(h, self, None)
         r._keep = keep
+        r.device = device
         return r
 
     def agg_finish(self, device: int, local_bits: Sequence[int]) -> List[int]:
@@ -421,18 +423,33 @@ class Block:
         return Block(h, n_rows, device, keep)
 
     @staticmethod
-    def wrap_device(device: int, ptr_cols: Sequence[tuple], n_rows: int) -> "Block":
-        """ptr_cols: (type, data_ptr, offsets_ptr or 0, data_bytes) with device addresses."""
+    def wrap_device(device: int, ptr_cols: Sequence[tuple], n_rows: int, keep=None) -> "Block":
+        """ptr_cols: (type, data_ptr, offsets_ptr or 0, data_bytes[, valid_ptr or 0]) with device addresses; `keep` is held as long
+        as the block (the owner of the memory)."""
         init([device])
         arr = (CColumn * max(len(ptr_cols), 1))()
-        for i, (t, dp, op, nb) in enumerate(ptr_cols):
+        for i, (t, dp, op, nb, *vp) in enumerate(ptr_cols):
             arr[i].type = t
             arr[i].data = dp
             arr[i].offsets = op or None
             arr[i].data_bytes = nb
+            arr[i].valid = (vp[0] if vp else 0) or None
         h = ct.c_void_p()
         _check(lib().tplx_gpu_block_wrap_device(device, arr, len(ptr_cols), n_rows, ct.byref(h)), "tplx_gpu_block_wrap_device")
-        return Block(h, n_rows, device)
+        return Block(h, n_rows, device, keep)
+
+    @staticmethod
+    def concat(parts: Sequence["Block"]) -> "Block":
+        """The rows of `parts` in order as one new block that owns its memory (tplx_gpu_block_concat); the parts may be freed
+        afterwards."""
+        if parts:
+            init([parts[0].device])
+        arr = (ct.c_void_p * max(len(parts), 1))(*[p._h for p in parts])
+        h = ct.c_void_p()
+        _check(lib().tplx_gpu_block_concat(arr, len(parts), ct.byref(h)), "tplx_gpu_block_concat")
+        nr = ct.c_uint64()
+        _check(lib().tplx_gpu_block_rows(h, ct.byref(nr)), "tplx_gpu_block_rows")
+        return Block(h, nr.value, parts[0].device if parts else 0)
 
     @staticmethod
     def from_partitions(device: int, partitions: Sequence[bytes], col_types: Sequence[int], option_cols: Sequence[int] = ()) -> "Block":
@@ -483,6 +500,8 @@ class Result:
         self._info = None
         self.hash_result = hash_result
         self._types = types  # results that do not come from a stage (join probe): the output column types
+        self._rowidx: Optional[bool] = None
+        self.device = block.device if block is not None else None
 
     @property
     def info(self) -> CResultInfo:
@@ -531,6 +550,29 @@ class Result:
 
     def columns(self) -> List[Column]:
         return [self.column(c) for c in range(len(self.out_types()))]
+
+    def as_block(self, n_cols: Optional[int] = None) -> Block:
+        """The first `n_cols` visible output columns (default: all but a stage's trailing __rowidx) as a block, with their
+        validity bitmaps, without a copy; the block keeps this result alive."""
+        types = self.out_types()
+        if n_cols is None:
+            n_cols = len(types) - (1 if self.rowidx else 0)
+        n = int(self.info.n_out_rows)
+        cols = []
+        for c in range(n_cols):
+            dp, op = self.device_column(c)
+            w = ct.c_void_p()
+            _check(lib().tplx_gpu_result_device_validity(self._h, c, ct.byref(w)), "result_device_validity")
+            cols.append((types[c], dp, op, int(self.info.out_str_bytes[c]) if types[c] == T_STR else n * 8, w.value or 0))
+        return Block.wrap_device(self.device, cols, n, keep=self)
+
+    @property
+    def rowidx(self) -> bool:
+        """The last visible output column is the stage's __rowidx (input row numbers), not a user column."""
+        if self._rowidx is None:
+            p = self.stage.program if self.stage is not None else None
+            self._rowidx = bool(p is not None and not self.hash_result and p.out_names[len(self.out_types()) - 1:len(self.out_types())] == ["__rowidx"])
+        return self._rowidx
 
     def device_column(self, c: int):
         d, o = ct.c_void_p(), ct.c_void_p()
@@ -586,7 +628,9 @@ class Result:
         arr = (ct.c_int64 * max(len(row_nos), 1))(*[int(v) for v in row_nos])
         h = ct.c_void_p()
         _check(lib().tplx_gpu_result_merge_resolved(self._h, resolved._h, arr, first_row_no, ct.byref(h)), "tplx_gpu_result_merge_resolved")
-        return Result(h, None, resolved, types=self.out_types())
+        r = Result(h, None, resolved, types=self.out_types())
+        r._rowidx = self.rowidx
+        return r
 
     def exception_partition(self) -> bytes:
         need = ct.c_uint64()

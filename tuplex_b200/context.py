@@ -58,6 +58,7 @@ class Metrics:
         self.csv_parse_ms = 0.0
         self.text_rows = 0  # lines the device text source split
         self.text_parse_ms = 0.0
+        self.device_handoff_rows = 0  # rows passed from one operator to the next as device blocks (join sides and outputs)
 
     def _add(self, info):
         self.rows_in += int(info.n_in_rows)

@@ -32,6 +32,7 @@
 #include "join.cuh"
 #include "option.cuh"
 #include "merge.cuh"
+#include "concat.cuh"
 #include "jit.inl"
 
 using namespace tplx;
@@ -1679,7 +1680,7 @@ static int32_t run_rows(tplx_stage *s, StageDev *sd, const tplx_block *b, int64_
                 oc.cap_bytes = cap_bytes[c];
                 rc = dalloc(r, &oc.offsets, cap_rows + 1);
                 if (rc) return rc;
-                rc = dalloc(r, &oc.bytes, cap_bytes[c]);
+                rc = dalloc(r, &oc.bytes, align_up(cap_bytes[c], 16) + 16);  // strops.cuh contract: readable to the next 16-byte boundary
                 if (rc) return rc;
                 oc.data = nullptr;
             } else {
@@ -2334,3 +2335,4 @@ extern "C" int32_t tplx_gpu_result_fetch_aggregate(tplx_result *r, int64_t *acc_
 #include "tplx_gpu_comm.inl"
 #include "tplx_gpu_join.inl"
 #include "tplx_gpu_merge.inl"
+#include "tplx_gpu_concat.inl"

@@ -52,11 +52,19 @@ class Source:
         self.total_rows = total_rows
 
     @property
+    def col_types(self) -> List[int]:
+        return [c.type for c in self.cols]
+
+    @property
     def option_cols(self) -> List[int]:
         return _option_cols(self.cols)
 
     def cost(self) -> int:
         return int(self.total_rows)
+
+    def to_host_source(self) -> "Source":
+        """The whole input as a host Source (stages whose UDFs are outside the GPU op set)."""
+        return self
 
 
 class FileSource(Source):
@@ -88,8 +96,86 @@ class FileSource(Source):
         raise NotImplementedError
 
     def to_host_source(self) -> Source:
-        """The whole input as a host Source (stages whose UDFs are outside the GPU op set)."""
         raise NotImplementedError
+
+
+class DeviceRows:
+    """Rows that pass from one operator to the next as device column blocks: the per-block results of one device (stage results,
+    their K9 merges with resolved rows, join probes) in row order, each with the visible columns `types` first. rows() turns them
+    into exactly the rows the host path produces from the same results."""
+
+    def __init__(self, parts: list, names: List[Optional[str]], types: List[int]):
+        self.parts, self.names, self.types = parts, list(names), list(types)
+        self.n_rows = sum(int(p.info.n_out_rows) for p in parts)
+        self.device = parts[0].device if parts else None
+
+    def nullable(self, c: int) -> bool:
+        return any(p.validity(c) is not None for p in self.parts)
+
+    def none_column(self) -> bool:
+        """Some column is None in every row: the host path types such a column from its values, not from the stage, so a consumer
+        that depends on types (a stage, a join) takes these rows on the host path."""
+        if self.n_rows == 0:
+            return False
+        for c in range(len(self.types)):
+            vs = [p.validity(c) for p in self.parts]
+            if any(v is not None for v in vs) and not any(v is None or v.any() for p, v in zip(self.parts, vs) if int(p.info.n_out_rows)):
+                return True
+        return False
+
+    def columns(self, part) -> List[Column]:
+        return [part.column(c) for c in range(len(self.types))]
+
+    def rows(self) -> list:
+        """Python rows (a value per row for one column), fetched once; the device results are released."""
+        vals: List[list] = [[] for _ in self.types]
+        for p in self.parts:
+            for acc, col in zip(vals, self.columns(p)):
+                acc.extend(col.to_values())
+        self.free()
+        if len(vals) == 1:
+            return vals[0]
+        return list(zip(*vals))
+
+    def csv(self, null_value: str) -> Optional[List[bytes]]:
+        """CSV text of every part on the device (K7); None when a part needs the host writer."""
+        chunks = [p.csv_bytes(n_cols=len(self.types), null_value=null_value) for p in self.parts]
+        return None if any(c is None for c in chunks) else chunks
+
+    def free(self):
+        for p in self.parts:
+            p.free()
+        self.parts = []
+
+
+class DeviceSource(Source):
+    """Input of a plan that another operator left on the device (a join's output): its parts run through the stage as blocks."""
+
+    def __init__(self, ctx, rows: DeviceRows):
+        super().__init__([], rows.names, rows.n_rows, None, [], rows.n_rows)
+        self.ctx, self.rows = ctx, rows
+
+    @property
+    def col_types(self) -> List[int]:
+        return list(self.rows.types)
+
+    @property
+    def option_cols(self) -> List[int]:
+        return [c for c in range(len(self.rows.types)) if self.rows.nullable(c)]
+
+    def to_host_source(self) -> Source:
+        return self.ctx._source_from_rows(self.rows.rows(), self.names)
+
+
+def _handoff_ok(ctx) -> bool:
+    """Stage and join results may stay on the device between operators: one device (a join's build side would otherwise need
+    copies between devices) and None kept in the normal case (the join consumes Option columns)."""
+    return len(ctx._devices) == 1 and ctx._options.get("tuplex.gpu.optionColumns", "true") == "true"
+
+
+def _count_handoff(ctx, n: int):
+    with _metrics_lock:
+        ctx.metrics.device_handoff_rows += int(n)
 
 
 class JoinSpec:
@@ -336,16 +422,30 @@ class DataSet:
                 pass
         return _map_output_names(op.udf, names)
 
-    def _execute(self, csv_sink: Optional[list] = None, csv_null: str = ""):
+    def _execute(self, csv_sink: Optional[list] = None, csv_null: str = "", handoff: bool = False):
         """Split the operator chain into stages and run them. Returns (python rows, column names). With `csv_sink` (a list) the
-        last stage may instead write its rows there as CSV text, None cells as `csv_null`, and return (None, column names)."""
+        last stage may instead write its rows there as CSV text, None cells as `csv_null`, and return (None, column names). With
+        `handoff` (the consumer is a join) a last row stage may instead return its results on the device, as a DeviceRows."""
         src = self._source
         self._last_exceptions = Counter()
         if self._join is not None:
-            rows, names = _run_join(self._ctx, self._join, self._last_exceptions)
+            rows, names = _run_join(self._ctx, self._join, self._last_exceptions, handoff or csv_sink is not None or bool(self._ops))
+            if isinstance(rows, DeviceRows):
+                if not self._ops:
+                    if handoff:
+                        return rows, names
+                    chunks = rows.csv(csv_null) if csv_sink is not None else None
+                    if chunks is not None:
+                        _count_handoff(self._ctx, rows.n_rows)
+                        rows.free()
+                        csv_sink.extend(chunks)
+                        return None, names
+                    return rows.rows(), names
+                if rows.none_column():
+                    rows = rows.rows()
             if not self._ops:
                 return rows, names
-            src = self._ctx._source_from_rows(rows, names)
+            src = DeviceSource(self._ctx, rows) if isinstance(rows, DeviceRows) else self._ctx._source_from_rows(rows, names)
         elif self._parent is not None:
             rows, names = self._parent._execute()
             src = self._ctx._source_from_rows(rows, names)
@@ -361,7 +461,8 @@ class DataSet:
             if si > 0:
                 src = self._ctx._source_from_rows(rows, names)
             last = si == len(stages) - 1
-            rows, names = _run_stage(self._ctx, src, ops, self._last_exceptions, csv_sink=csv_sink if last else None, csv_null=csv_null)
+            rows, names = _run_stage(self._ctx, src, ops, self._last_exceptions, csv_sink=csv_sink if last else None, csv_null=csv_null,
+                                     handoff=handoff and last)
         return rows, names
 
 
@@ -426,7 +527,7 @@ def _option_cols(cols) -> List[int]:
 def _compile_row_ops(src: Source, ops: Sequence[Op]) -> StageCompiler:
     """A stage compiler over `src`'s columns fed the row operators `ops`; UnsupportedUDF for a UDF outside the GPU op set and
     for any operator that is not a row operator."""
-    sc = StageCompiler([c.type for c in src.cols], src.names, src.option_cols)
+    sc = StageCompiler(src.col_types, src.names, src.option_cols)
     for op in ops:
         if op.kind == "map":
             sc.add_map(op.udf, op.id)
@@ -464,17 +565,26 @@ def _rows_as_tuples(rows):
     return [r if isinstance(r, tuple) else (r,) for r in rows]
 
 
-def _run_join(ctx, spec: JoinSpec, exc_counter: Counter):
+def _run_join(ctx, spec: JoinSpec, exc_counter: Counter, handoff: bool = False):
     """A JoinOperator between two executed datasets: HashJoinStage of the reference (core/src/physical/HashJoinStage.cc; build stage
     with a hash-table endpoint + probe inside the other side's pipeline, PipelineBuilder.cc:2110-2523) on the GPU (K8,
-    tplx_gpu_join_build / tplx_gpu_join_probe). Rows outside the normal case of either side (fallback rows) are joined on the
-    interpreter path and merged by (probe row, build row), which is the order the normal case produces."""
-    lrows, lnames = spec.left._execute()
-    rrows, rnames = spec.right._execute()
+    tplx_gpu_join_build / tplx_gpu_join_probe). Sides that a stage or join left on the device are joined there (_device_join);
+    otherwise every side comes to the host as rows and rows outside the normal case of either side (fallback rows) are joined on
+    the interpreter path and merged by (probe row, build row), which is the order the normal case produces. With `handoff` the
+    output may stay on the device (DeviceRows)."""
+    ok = _handoff_ok(ctx)
+    left, lnames = spec.left._execute(handoff=ok)
+    right, rnames = spec.right._execute(handoff=ok)
     exc_counter.update(spec.left._last_exceptions)
     exc_counter.update(spec.right._last_exceptions)
     lnames = list(lnames) if lnames else []
     rnames = list(rnames) if rnames else []
+    if ok:
+        out = _device_join(ctx, spec, left, lnames, right, rnames, handoff)
+        if out is not None:
+            return out
+    lrows = left.rows() if isinstance(left, DeviceRows) else left
+    rrows = right.rows() if isinstance(right, DeviceRows) else right
     li, ri = spec.key_indices(lnames, rnames)
     names = spec.names(lnames, rnames)
     build_right = spec.build_right()
@@ -582,6 +692,85 @@ def _run_join(ctx, spec: JoinSpec, exc_counter: Counter):
     return rows, names
 
 
+def _device_join(ctx, spec: JoinSpec, left, lnames, right, rnames, handoff: bool):
+    """The join of two sides of which at least one is on the device (DeviceRows), without bringing it to the host: the build
+    side is one block (a single result wrapped, several concatenated on the device), the probe side's results are probed in
+    order; a host side is uploaded as on the host path. None (nothing run) where only the host path gives the answer: a
+    column that is None in every row, an empty host side, fallback rows on a host side, key types that differ or are f64, too many
+    columns."""
+    sides = [(left, lnames), (right, rnames)]
+    if not any(isinstance(s, DeviceRows) for s, _ in sides):
+        return None
+    li, ri = spec.key_indices(lnames, rnames)
+    names = spec.names(lnames, rnames)
+    types, host_srcs = [], []
+    for s, nm in sides:
+        if isinstance(s, DeviceRows):
+            if s.none_column() or len(s.types) != len(nm):
+                return None
+            types.append(s.types)
+            host_srcs.append(None)
+        else:
+            if not s:
+                return None
+            hs = ctx._source_from_rows(s, nm, option=True)
+            if hs.fallback or len(hs.cols) != len(nm):
+                return None
+            types.append(hs.col_types)
+            host_srcs.append(hs)
+    if types[0][li] != types[1][ri] or types[0][li] == T_F64 or len(names) > C["TPLX_MAX_COLS"] - 2:
+        return None
+    build_right = spec.build_right()
+    left_outer = spec.kind == "left"
+    dev = next(s.device for s, _ in sides if isinstance(s, DeviceRows))
+    backend.init([dev])
+    pi, bi = (0, 1) if build_right else (1, 0)
+    pk, bk = (li, ri) if build_right else (ri, li)
+
+    def blocks(i: int, one: bool) -> list:
+        """Side i as device blocks in row order: its results wrapped, or its host columns uploaded (one block, or blocks of
+        tuplex.gpu.blockRows rows)."""
+        s, hs = sides[i][0], host_srcs[i]
+        if hs is None:
+            return [p.as_block(len(s.types)) for p in s.parts]
+        n, step = hs.n_rows, (hs.n_rows if one else ctx._block_rows)
+        return [backend.Block.upload(dev, [c.slice(lo, min(n, lo + step)) for c in hs.cols], min(n, lo + step) - lo) for lo in range(0, n, step)]
+
+    for s, _ in sides:
+        if isinstance(s, DeviceRows):
+            _count_handoff(ctx, s.n_rows)
+    bparts = blocks(bi, True)
+    if len(bparts) == 1:
+        bb = bparts[0]
+    else:
+        import time
+        t0 = time.perf_counter()
+        bb = backend.Block.concat(bparts)
+        with _metrics_lock:
+            ctx.metrics.join_concat_ms = getattr(ctx.metrics, "join_concat_ms", 0.0) + (time.perf_counter() - t0) * 1e3
+            ctx.metrics.join_concat_bytes = getattr(ctx.metrics, "join_concat_bytes", 0) + sum(
+                int(p.info.n_out_rows) * 8 if t != T_STR else int(p.info.out_str_bytes[c]) + int(p.info.n_out_rows) * 4
+                for p in sides[bi][0].parts for c, t in enumerate(types[bi]))
+        del bparts
+    jn = backend.Join(bb, types[bi], bk)
+    outs = []
+    for pb in blocks(pi, False):
+        res = jn.probe(pb, types[pi], pk, left_outer=left_outer, build_first=not build_right)
+        with _metrics_lock:
+            ctx.metrics._add(res.info)
+            ctx.metrics.join_probe_rows = getattr(ctx.metrics, "join_probe_rows", 0) + pb.n_rows
+        outs.append(res)
+    with _metrics_lock:
+        ctx.metrics.join_build_ms = getattr(ctx.metrics, "join_build_ms", 0.0) + jn.info["build_ms"]
+    jn.free()
+    bb.free()
+    for s, _ in sides:
+        if isinstance(s, DeviceRows):
+            s.free()
+    out = DeviceRows(outs, names, outs[0].out_types() if outs else [])
+    return (out if handoff else out.rows()), names
+
+
 def _join_row(lrow, li, rrow, ri, n_right_cols):
     rr = rrow if rrow is not None else (None,) * n_right_cols
     return tuple(v for i, v in enumerate(lrow) if i != li) + (lrow[li],) + tuple(v for i, v in enumerate(rr) if i != ri)
@@ -636,8 +825,10 @@ def _py_join_pairs(L, li, R, ri, left_outer, build_right, n_right_cols):
     return out
 
 
-def _run_stage(ctx, src: Source, ops: List[Op], exc_counter: Counter, csv_sink: Optional[list] = None, csv_null: str = ""):
-    """One TransformStage on the GPU + CPython resolve of its exception rows."""
+def _run_stage(ctx, src: Source, ops: List[Op], exc_counter: Counter, csv_sink: Optional[list] = None, csv_null: str = "",
+               handoff: bool = False):
+    """One TransformStage on the GPU + CPython resolve of its exception rows. With `handoff` a row stage returns its results on
+    the device (DeviceRows) when they can stay there."""
     end = ops[-1] if ops and ops[-1].kind in _ENDPOINTS else None
     row_ops = ops[:-1] if end else ops
     is_file = isinstance(src, FileSource)  # the device parses the file right in front of the stage
@@ -647,14 +838,17 @@ def _run_stage(ctx, src: Source, ops: List[Op], exc_counter: Counter, csv_sink: 
         plan = _compile_stage(src, row_ops, end)
     except UnsupportedUDF as e:
         ctx._log(f"stage falls back to the CPython path: {e}")
-        return _run_stage_python(src.to_host_source() if is_file else src, ops, exc_counter)
+        return _run_stage_python(src.to_host_source(), ops, exc_counter)
     backend.init(sorted(set(ctx._devices)))
     stage = backend.Stage(plan.prog)
-    hold = csv_sink is not None
-    shards = [_file_blocks(ctx, plan, stage, src, hold)] if is_file else _column_blocks(ctx, plan, stage, src, hold)
+    hold = csv_sink is not None or handoff
+    if isinstance(src, DeviceSource):
+        shards = [_device_blocks(ctx, plan, stage, src, hold)]
+    else:
+        shards = [_file_blocks(ctx, plan, stage, src, hold)] if is_file else _column_blocks(ctx, plan, stage, src, hold)
     st = _stitch(shards, src.fallback)
     if end is None:
-        rows, names = _rows_endpoint(plan, st, src, exc_counter, csv_sink, csv_null), plan.out_names
+        rows, names = _rows_endpoint(plan, st, src, exc_counter, csv_sink, csv_null, handoff), plan.out_names
     elif end.kind == "aggregate":
         rows, names = _aggregate_endpoint(plan, st, src.names, exc_counter)
     else:
@@ -786,6 +980,37 @@ def _file_blocks(ctx, plan: _StagePlan, stage, src: FileSource, hold: bool) -> _
     return sh
 
 
+def _device_blocks(ctx, plan: _StagePlan, stage, src: DeviceSource, hold: bool) -> _Shard:
+    """The block loop over rows another operator left on the device: every part runs as a block, row numbering carried on as in
+    _column_blocks. Rows whose UDF raised get their input row from that part's fetched columns, for those rows only."""
+    rows = src.rows
+    sh = _Shard(rows.device)
+    lo = 0
+    for part in rows.parts:
+        n = int(part.info.n_out_rows)
+        res = stage.run(part.as_block(len(rows.types)), sh.row_no)
+        exc = res.exceptions()
+        if len(exc):
+            cols = rows.columns(part)
+            for r in exc["row"]:
+                vals = tuple(_value_at(c, int(r)) for c in cols)
+                sh.inputs[lo + int(r)] = vals if len(vals) != 1 else vals[0]
+        sh.take(ctx, plan, res, lo, exc, None, hold)
+        lo += n
+    _count_handoff(ctx, lo)
+    return sh
+
+
+def _value_at(col: Column, i: int):
+    """Python value of row i of a fetched column, as Column.to_values gives it."""
+    if col.valid is not None and not (int(col.valid[i >> 5]) >> (i & 31)) & 1:
+        return None
+    if col.type == T_STR:
+        return col.data[int(col.offsets[i]):int(col.offsets[i + 1])].tobytes().decode("utf-8", "replace")
+    v = col.data[i].item()
+    return bool(v) if col.type == T_BOOL else v
+
+
 def _column_blocks(ctx, plan: _StagePlan, stage, src: Source, hold: bool) -> List[_Shard]:
     """The block loop of a column source: blocks are sharded contiguously over the context's devices (tuplex.gpu.devices), one
     task per device, its blocks in order; concatenating the shards in device order preserves the input order
@@ -846,29 +1071,36 @@ def _stitch(shards: List[_Shard], fallback: List[Tuple[int, Any]]) -> _Shard:
     return st
 
 
-def _rows_endpoint(plan: _StagePlan, st: _Shard, src: Source, exc_counter: Counter, csv_sink: Optional[list], csv_null: str = ""):
+def _rows_endpoint(plan: _StagePlan, st: _Shard, src: Source, exc_counter: Counter, csv_sink: Optional[list], csv_null: str = "",
+                   handoff: bool = False):
     """Memory endpoint: the normal-case rows with the rows resolved on the CPython path merged in, in order. With a CSV sink
-    the device writes the text into `csv_sink` when it can, and None is returned."""
+    the device writes the text into `csv_sink` when it can, and None is returned; with `handoff` the results stay on the device
+    when they can and a DeviceRows is returned."""
     prog, row_ops = plan.prog, plan.row_ops
     ncols = len(prog.out_cols) - prog.hidden_out_cols
     user_cols = ncols - (1 if plan.need_rowidx else 0)
     excs = st.exceptions()
-    if csv_sink is not None:
-        # the device row writer (K7) prints None cells as `csv_null`. Exception rows resolved in CPython go back into their slots
-        # ON THE DEVICE (K9, ResolveTask::executeInOrder), except when they must merge with fallback rows by __rowidx
-        chunks = None
-        if not st.fallback and not (len(excs) and plan.need_rowidx):
-            option_outs = {k - 1 for k in prog.out_null_of if k}
-            chunks = _device_merge_csv(st.held, row_ops, src.names, st.inputs, [t for _, t in prog.out_cols[:user_cols]], option_outs,
-                                       csv_null, exc_counter)
-        if chunks is not None:
-            csv_sink.extend(chunks)
-            for res, *_ in st.held:
-                res.free()
-            return None
-        for res, lo, rowmap, *_ in st.held:
-            st.out_cols.append(plan.fetch_cols(res, lo, rowmap))
-            res.free()
+    if (csv_sink is not None or handoff) and not st.fallback:
+        # Exception rows resolved in CPython go back into their slots ON THE DEVICE (K9, ResolveTask::executeInOrder), except when
+        # they must merge with fallback rows by __rowidx. The device row writer (K7) prints None cells as `csv_null`.
+        if csv_sink is not None:
+            chunks = _device_merge_csv(plan, st.held, src.names, st.inputs, csv_null, exc_counter)
+            if chunks is not None:
+                csv_sink.extend(chunks)
+                for res, *_ in st.held:
+                    res.free()
+                return None
+        else:
+            parts, counts = _device_merge(plan, st.held, src.names, st.inputs)
+            if parts is not None:
+                exc_counter.update(counts)
+                for res, *_ in st.held:
+                    if not any(p is res for p in parts):
+                        res.free()
+                return DeviceRows(parts, plan.out_names, [t for _, t in prog.out_cols[:user_cols]])
+    for res, lo, rowmap, *_ in st.held:
+        st.out_cols.append(plan.fetch_cols(res, lo, rowmap))
+        res.free()
     merged_vals = [sum((oc[c].to_values() for oc in st.out_cols), []) for c in range(ncols)]
     n_out = len(merged_vals[0]) if ncols else 0
     normal_rows = [tuple(merged_vals[c][i] for c in range(user_cols)) if user_cols != 1 else merged_vals[0][i] for i in range(n_out)]
@@ -1030,41 +1262,62 @@ def _fits_type(v, t: int) -> bool:
     return isinstance(v, int) and not isinstance(v, bool) and -(1 << 63) <= v < (1 << 63)
 
 
-def _device_merge_csv(held, row_ops, names, inputs: Dict[int, Any], out_types, option_outs, null_value: str,
-                      exc_counter: Counter) -> Optional[List[bytes]]:
-    """CSV text of every held block result with its resolved exception rows merged in order on the device
-    (tplx_gpu_result_merge_resolved + tplx_gpu_result_csv_nulls; None cells of the Option output columns `option_outs` are written
-    as `null_value`). None when a resolved row does not fit the stage's output schema (the host path then merges and formats);
-    exception counts are only taken over on success."""
-    ncols = len(out_types)
-    chunks: List[bytes] = []
+def _device_merge(plan: _StagePlan, held, names, inputs: Dict[int, Any]):
+    """(every held block result with its resolved exception rows merged in order on the device (tplx_gpu_result_merge_resolved),
+    the exception counts of the resolve). A result without exception rows is its own part. (None, None) when a resolved row does
+    not fit the stage's output schema: the host path then merges, and counts the exceptions itself. A stage with __rowidx gets
+    each resolved row's block row there (its input row: no fallback rows, so the order of row numbers is the input order)."""
+    prog = plan.prog
+    ncols = len(prog.out_cols) - prog.hidden_out_cols
+    user_cols = ncols - (1 if plan.need_rowidx else 0)
+    out_types = [t for _, t in prog.out_cols[:ncols]]
+    option_outs = {k - 1 for k in prog.out_null_of if k}
+    parts: list = []
     counts: Counter = Counter()
+
+    def give_up():
+        for p in parts:
+            if not any(p is res for res, *_ in held):
+                p.free()
+        return None, None
+
     for res, lo, _rowmap, frn, dev in held:
         ex = res.exceptions()
         if not len(ex):
-            txt = res.csv_bytes(n_cols=ncols, null_value=null_value)
-            if txt is None:
-                return None
-            chunks.append(txt)
+            parts.append(res)
             continue
         rows, nos = [], []
         for e in ex[np.argsort(ex["row_no"], kind="stable")]:
-            r = _run_py(row_ops, inputs[lo + int(e["row"])], names, counts, int(e["op_id"]))
+            r = _run_py(plan.row_ops, inputs[lo + int(e["row"])], names, counts, int(e["op_id"]))
             if r is None:
                 continue
             vt = r[0] if isinstance(r[0], tuple) else (r[0],)
-            if len(vt) != ncols or not all(_fits_type(v, t) or (v is None and c in option_outs) for c, (v, t) in enumerate(zip(vt, out_types))):
-                return None
-            rows.append(vt)
+            if len(vt) != user_cols or not all(_fits_type(v, t) or (v is None and c in option_outs) for c, (v, t) in enumerate(zip(vt, out_types))):
+                return give_up()
+            rows.append(vt + ((int(e["row"]),) if plan.need_rowidx else ()))
             nos.append(int(e["row_no"]))
+        if not rows:  # nothing resolved: the result already leaves every exception's slot empty
+            parts.append(res)
+            continue
         blk = backend.Block.upload(dev, [Column.from_values([r[c] for r in rows], out_types[c]) for c in range(ncols)], len(rows))
-        merged = res.merge_resolved(blk, nos, frn)
-        txt = merged.csv_bytes(n_cols=ncols, null_value=null_value)
-        merged.free()
-        blk.free()
-        if txt is None:
-            return None
-        chunks.append(txt)
+        parts.append(res.merge_resolved(blk, nos, frn))
+    return parts, counts
+
+
+def _device_merge_csv(plan: _StagePlan, held, names, inputs: Dict[int, Any], null_value: str, exc_counter: Counter) -> Optional[List[bytes]]:
+    """CSV text of every held block result with its resolved exception rows merged in order on the device (_device_merge, then
+    tplx_gpu_result_csv_nulls; None cells of Option output columns are written as `null_value`). None when a resolved row does not
+    fit the stage's output schema or a part needs the host writer; exception counts are only taken over on success."""
+    parts, counts = _device_merge(plan, held, names, inputs)
+    if parts is None:
+        return None
+    ncols = len(plan.prog.out_cols) - plan.prog.hidden_out_cols - (1 if plan.need_rowidx else 0)
+    chunks = [p.csv_bytes(n_cols=ncols, null_value=null_value) for p in parts]
+    for p in parts:
+        if not any(p is res for res, *_ in held):
+            p.free()
+    if any(c is None for c in chunks):
+        return None
     exc_counter.update(counts)
     return chunks
 
