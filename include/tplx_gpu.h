@@ -152,6 +152,38 @@ int32_t tplx_gpu_block_free(tplx_block *block);
  * different devices or with different column counts / types: TPLX_E_BADARG; a string column above 4 GiB: TPLX_E_OVERFLOW. Zero
  * parts give an empty block with no columns on the first initialised device. The parts may be freed when the call returns. */
 int32_t tplx_gpu_block_concat(const tplx_block *const *parts, uint32_t n_parts, tplx_block **out);
+/* Rows [first_row, first_row + n_rows) of `block`: one piece of tplx_gpu_block_concat_pieces. */
+typedef struct tplx_concat_piece {
+    const tplx_block *block;
+    uint64_t first_row;
+    uint64_t n_rows;
+} tplx_concat_piece;
+/* Per-column flags of tplx_gpu_block_concat_pieces (0 = the column as tplx_gpu_block_concat makes it). */
+enum tplx_concat_flags {
+    TPLX_CONCAT_DROP_VALID = 1, /* no bitmap in the output: the caller has counted no None in the pieces' rows */
+    TPLX_CONCAT_ALL_NONE = 2,   /* None in every row: the output column is TPLX_T_I64 zeros with every validity bit clear; the
+                                   pieces' values are not read */
+    TPLX_CONCAT_UTF8 = 4,       /* string column: every string is written as CPython's bytes.decode("utf-8", "replace").encode()
+                                   gives it (one U+FFFD per maximal invalid subpart); valid strings keep their bytes */
+};
+/* tplx_gpu_block_concat over row ranges of blocks: the rows of every piece, in order, as one new block that owns its memory.
+ * String offsets are rebased from each piece's first offset and validity words realigned from its first row. `col_flags` holds one
+ * tplx_concat_flags value per column, or is NULL (all 0). A piece outside its block, or TPLX_CONCAT_UTF8 on a column that is not a
+ * string column: TPLX_E_BADARG. A device allocation that fails: TPLX_E_NOMEM, nothing is kept. Other errors as
+ * tplx_gpu_block_concat; a string column above 4 GiB after the replacement is TPLX_E_OVERFLOW. The blocks may be freed when the call
+ * returns. This is how DataSet.cache() re-blocks stage results into owned blocks. */
+int32_t tplx_gpu_block_concat_pieces(const tplx_concat_piece *pieces, uint32_t n_pieces, const uint8_t *col_flags, tplx_block **out);
+/* Column statistics of a block (one launch over all columns): none_rows[c] = rows in [0, n_rows) whose validity bit is clear
+ * (bits past n_rows are ignored; 0 for a column without a bitmap); invalid_utf8[c] = strings of a string column that
+ * TPLX_CONCAT_UTF8 would change, found by validating only the strings of 1024-row tiles whose bytes are not all ASCII (0 for
+ * other columns). Both arrays have one entry per column. */
+int32_t tplx_gpu_block_stats(const tplx_block *block, uint64_t *none_rows, uint64_t *invalid_utf8);
+/* Copy column `col` of a device-resident block to the host: fixed width -> data (n_rows * 8 bytes); TPLX_T_STR -> data (the
+ * column's bytes) and offsets (n_rows + 1). data or offsets may be NULL. The block twin of tplx_gpu_result_fetch_column. */
+int32_t tplx_gpu_block_fetch_column(const tplx_block *block, uint32_t col, void *data, uint32_t *offsets);
+/* A block over the same device memory as `block` that owns none of it (freeing it frees nothing of `block`); `block` must
+ * outlive it. Lets a block that several consumers read (a cached dataset) go where the consumer frees its input block. */
+int32_t tplx_gpu_block_view(const tplx_block *block, tplx_block **out);
 
 /* ---- execution -------------------------------------------------------------------------- */
 /* Run the stage over one block (asynchronously on the device's stream; results are complete

@@ -19,10 +19,12 @@ from .ir import T_BOOL, T_F64, T_I64, T_STR
 
 _LIB_PATH = os.environ.get("TPLX_GPU_LIB") or os.path.join(os.path.dirname(os.path.abspath(__file__)), "lib", "libtplx_gpu.so")
 MAX_COLS = ir.C["TPLX_MAX_COLS"]
+E_NOMEM = -5  # TPLX_E_NOMEM
+CONCAT_DROP_VALID, CONCAT_ALL_NONE, CONCAT_UTF8 = 1, 2, 4  # tplx_concat_flags
 
 
 class GpuBackendError(RuntimeError):
-    pass
+    code = 0  # tplx_status of the failed call (0 = not from the C ABI)
 
 
 class CColumn(ct.Structure):
@@ -50,6 +52,10 @@ class CCsvDesc(ct.Structure):
 class CCsvInfo(ct.Structure):
     _fields_ = [("n_rows", ct.c_uint64), ("n_normal", ct.c_uint64), ("n_bad", ct.c_uint64), ("sequential_rows", ct.c_uint32),
                 ("kernel_launches", ct.c_uint32), ("parse_ms", ct.c_double)]
+
+
+class CConcatPiece(ct.Structure):
+    _fields_ = [("block", ct.c_void_p), ("first_row", ct.c_uint64), ("n_rows", ct.c_uint64)]
 
 
 class CTextDesc(ct.Structure):
@@ -92,6 +98,10 @@ def lib():
         "tplx_gpu_block_fetch_validity": ([vp, u32, vp, P(u32)], i32),
         "tplx_gpu_block_free": ([vp], i32),
         "tplx_gpu_block_concat": ([P(vp), u32, P(vp)], i32),
+        "tplx_gpu_block_concat_pieces": ([P(CConcatPiece), u32, vp, P(vp)], i32),
+        "tplx_gpu_block_stats": ([vp, P(u64), P(u64)], i32),
+        "tplx_gpu_block_fetch_column": ([vp, u32, vp, vp], i32),
+        "tplx_gpu_block_view": ([vp, P(vp)], i32),
         "tplx_gpu_stage_run": ([vp, vp, i64, P(vp)], i32),
         "tplx_gpu_stage_run_host": ([vp, i32, P(CColumn), u32, u64, i64, P(vp)], i32),
         "tplx_gpu_result_info": ([vp, P(CResultInfo)], i32),
@@ -145,7 +155,9 @@ def lib():
 def _check(rc: int, what: str):
     if rc != 0:
         msg = lib().tplx_gpu_last_error().decode("utf-8", "replace")
-        raise GpuBackendError(f"{what} failed ({rc}): {msg}")
+        err = GpuBackendError(f"{what} failed ({rc}): {msg}")
+        err.code = rc
+        raise err
 
 
 _initialised: set = set()
@@ -450,6 +462,65 @@ class Block:
         nr = ct.c_uint64()
         _check(lib().tplx_gpu_block_rows(h, ct.byref(nr)), "tplx_gpu_block_rows")
         return Block(h, nr.value, parts[0].device if parts else 0)
+
+    @staticmethod
+    def concat_pieces(pieces: Sequence[tuple], col_flags: Optional[Sequence[int]] = None) -> "Block":
+        """Rows [first, first + n) of every (block, first, n) piece, in order, as one new block that owns its memory
+        (tplx_gpu_block_concat_pieces); `col_flags` holds one CONCAT_* combination per column (None: every column as concat makes
+        it). The blocks may be freed afterwards."""
+        if pieces:
+            init([pieces[0][0].device])
+        arr = (CConcatPiece * max(len(pieces), 1))()
+        for i, (b, first, n) in enumerate(pieces):
+            arr[i].block, arr[i].first_row, arr[i].n_rows = b._h, int(first), int(n)
+        flags = bytes(col_flags) if col_flags is not None else None
+        h = ct.c_void_p()
+        _check(lib().tplx_gpu_block_concat_pieces(arr, len(pieces), flags, ct.byref(h)), "tplx_gpu_block_concat_pieces")
+        nr = ct.c_uint64()
+        _check(lib().tplx_gpu_block_rows(h, ct.byref(nr)), "tplx_gpu_block_rows")
+        return Block(h, nr.value, pieces[0][0].device if pieces else 0)
+
+    def n_cols(self) -> int:
+        n = ct.c_uint32()
+        _check(lib().tplx_gpu_block_column_bytes(self._h, None, 0, ct.byref(n)), "tplx_gpu_block_column_bytes")
+        return n.value
+
+    def column_bytes(self) -> List[int]:
+        """Device bytes of every column: values, or string bytes + offsets (tplx_gpu_block_column_bytes); bitmaps not included."""
+        arr = (ct.c_uint64 * MAX_COLS)()
+        n = ct.c_uint32()
+        _check(lib().tplx_gpu_block_column_bytes(self._h, arr, MAX_COLS, ct.byref(n)), "tplx_gpu_block_column_bytes")
+        return [int(arr[i]) for i in range(n.value)]
+
+    def stats(self):
+        """(None rows, strings that are not valid UTF-8) per column, counted on the device (tplx_gpu_block_stats)."""
+        none, bad = (ct.c_uint64 * MAX_COLS)(), (ct.c_uint64 * MAX_COLS)()
+        _check(lib().tplx_gpu_block_stats(self._h, none, bad), "tplx_gpu_block_stats")
+        n = self.n_cols()
+        return [int(none[i]) for i in range(n)], [int(bad[i]) for i in range(n)]
+
+    def column(self, c: int, t: int) -> "Column":
+        """Column c (of type t) fetched to the host with its validity words, tail bits cleared (tplx_gpu_block_fetch_column)."""
+        n = int(self.n_rows)
+        valid = self.validity(c)
+        if valid is not None and n & 31:
+            valid[-1] &= np.uint32((1 << (n & 31)) - 1)
+        if t == T_STR:
+            offsets = np.empty(n + 1, dtype=np.uint32)
+            _check(lib().tplx_gpu_block_fetch_column(self._h, c, None, offsets.ctypes.data), "block_fetch_column")
+            data = np.empty(max(int(offsets[-1]), 1), dtype=np.uint8)
+            _check(lib().tplx_gpu_block_fetch_column(self._h, c, data.ctypes.data, None), "block_fetch_column")
+            return Column(T_STR, data[:int(offsets[-1])], offsets, valid)
+        data = np.empty(n, dtype=np.float64 if t == T_F64 else np.int64)
+        if n:
+            _check(lib().tplx_gpu_block_fetch_column(self._h, c, data.ctypes.data, None), "block_fetch_column")
+        return Column(t, data, None, valid)
+
+    def view(self) -> "Block":
+        """A block over this block's memory that owns none of it (tplx_gpu_block_view): freeing it leaves this block intact."""
+        h = ct.c_void_p()
+        _check(lib().tplx_gpu_block_view(self._h, ct.byref(h)), "tplx_gpu_block_view")
+        return Block(h, self.n_rows, self.device, keep=self)
 
     @staticmethod
     def from_partitions(device: int, partitions: Sequence[bytes], col_types: Sequence[int], option_cols: Sequence[int] = ()) -> "Block":

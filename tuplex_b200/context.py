@@ -59,6 +59,8 @@ class Metrics:
         self.text_rows = 0  # lines the device text source split
         self.text_parse_ms = 0.0
         self.device_handoff_rows = 0  # rows passed from one operator to the next as device blocks (join sides and outputs)
+        self.cache_rows = 0   # rows cache() placed in device blocks
+        self.cache_bytes = 0  # device bytes the cached datasets hold now (falls when a cache is freed)
 
     def _add(self, info):
         self.rows_in += int(info.n_in_rows)

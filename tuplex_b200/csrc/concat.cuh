@@ -1,22 +1,26 @@
-// concat.cuh — block concatenation: the rows of several device blocks, in order, as one block (tplx_gpu_block_concat).
+// concat.cuh — block concatenation: row ranges of several device blocks, in order, as one block (tplx_gpu_block_concat_pieces;
+// tplx_gpu_block_concat takes whole blocks).
 //
 // Used where one operator needs a single block of rows that an upstream stage produced as several block results (the build side
 // of a hash join, K8, takes exactly one block). Fixed-width columns and string bytes move with device-to-device copies; what
 // has to be rewritten per row runs as one batched launch per column over all parts:
-//   - string offsets: row i of part p gets its offset plus the bytes of the parts in front of p;
+//   - string offsets: row i of part p gets its offset less the part's first offset plus the bytes of the parts in front of p;
 //   - validity words: every output word is assembled from the (at most a few) parts whose rows it covers, each part's words
-//     realigned to the part's first output row with a funnel shift. Bits past a part's row count are never read into the
+//     realigned from the part's first row to its first output row with a funnel shift. Bits past a part's row count are never read into the
 //     output (results may carry garbage there); a part without a bitmap contributes set bits; the output's tail bits are zero.
 #pragma once
 #include <stdint.h>
 
 namespace tplx {
 
-// per (column, part) of a concat
+// per (column, part) of a concat; a part is rows [row0, row0 + its row count) of a block
 struct ConcatPart {
-    const uint32_t *offsets;  // string column: n_rows + 1 offsets into the part's bytes
-    const uint32_t *valid;    // validity words, or nullptr (every row holds a value)
+    const uint8_t *bytes;     // string column: the block's bytes
+    const uint32_t *offsets;  // string column: the block's offsets
+    const uint32_t *valid;    // validity words of the block, or nullptr (every row holds a value)
+    uint64_t row0;            // the part's first row in the block
     uint64_t byte_base;       // string column: output position of the part's first byte
+    uint64_t shift;           // string column: byte_base - offsets[row0], modulo 2^64
 };
 
 constexpr uint32_t CONCAT_NT = 256;
@@ -44,7 +48,7 @@ __global__ void __launch_bounds__(CONCAT_NT) concat_offsets_kernel(const ConcatP
     }
     const uint32_t p = concat_part_of(row_base, n_parts, i);
     const ConcatPart cp = parts[p];
-    out[i] = (uint32_t)(cp.offsets[i - row_base[p]] + cp.byte_base);
+    out[i] = (uint32_t)(cp.offsets[cp.row0 + i - row_base[p]] + cp.shift);
 }
 
 // out[w] for w < (n + 31) / 32: bits 32w .. 32w + 31 of the concatenated column's validity
@@ -64,9 +68,10 @@ __global__ void __launch_bounds__(CONCAT_NT) concat_valid_kernel(const ConcatPar
         const uint32_t *v = parts[p].valid;
         uint32_t bits = mask;
         if (v) {
-            const uint64_t wl = lo >> 5, wh = (hi - 1) >> 5;  // the part's words that hold rows lo .. hi - 1 (one or two)
+            const uint64_t sl = parts[p].row0 + lo, sh = parts[p].row0 + hi - 1;  // the block's rows
+            const uint64_t wl = sl >> 5, wh = sh >> 5;  // the block's words that hold them (one or two)
             const uint32_t a = v[wl], c = wh != wl ? v[wh] : 0u;
-            bits = __funnelshift_r(a, c, (uint32_t)(lo & 31)) & mask;
+            bits = __funnelshift_r(a, c, (uint32_t)(sl & 31)) & mask;
         }
         word |= bits << (uint32_t)(b + lo - r0);
     }

@@ -33,6 +33,7 @@
 #include "option.cuh"
 #include "merge.cuh"
 #include "concat.cuh"
+#include "cache.cuh"
 #include "jit.inl"
 
 using namespace tplx;

@@ -12,6 +12,7 @@ them on the CPython path, merge in order.
 from __future__ import annotations
 
 import threading
+import weakref
 from collections import Counter
 from concurrent.futures import ThreadPoolExecutor
 from typing import Any, Dict, List, Optional, Sequence, Tuple
@@ -101,27 +102,34 @@ class FileSource(Source):
 
 class DeviceRows:
     """Rows that pass from one operator to the next as device column blocks: the per-block results of one device (stage results,
-    their K9 merges with resolved rows, join probes) in row order, each with the visible columns `types` first. rows() turns them
-    into exactly the rows the host path produces from the same results."""
+    their K9 merges with resolved rows, join probes) or the blocks of a cached dataset, in row order, each with the visible columns
+    `types` first. rows() turns them into exactly the rows the host path produces from the same results. Owned parts are freed by
+    free() (a consumer takes them once); borrowed parts (a cache's blocks) belong to someone else and free() leaves them."""
 
-    def __init__(self, parts: list, names: List[Optional[str]], types: List[int]):
-        self.parts, self.names, self.types = parts, list(names), list(types)
+    def __init__(self, parts: list, names: List[Optional[str]], types: List[int], owned: bool = True):
+        self.parts, self.names, self.types, self.owned = parts, list(names), list(types), owned
         self.n_rows = sum(int(p.info.n_out_rows) for p in parts)
         self.device = parts[0].device if parts else None
 
     def nullable(self, c: int) -> bool:
         return any(p.validity(c) is not None for p in self.parts)
 
+    def stats(self) -> List[Tuple[List[int], List[int]]]:
+        """(None rows, strings that are not valid UTF-8) per column of every part, counted on the device (tplx_gpu_block_stats)."""
+        out = []
+        for p in self.parts:
+            b = p.as_block(len(self.types))
+            out.append(b.stats())
+            b.free()
+        return out
+
     def none_column(self) -> bool:
         """Some column is None in every row: the host path types such a column from its values, not from the stage, so a consumer
         that depends on types (a stage, a join) takes these rows on the host path."""
         if self.n_rows == 0:
             return False
-        for c in range(len(self.types)):
-            vs = [p.validity(c) for p in self.parts]
-            if any(v is not None for v in vs) and not any(v is None or v.any() for p, v in zip(self.parts, vs) if int(p.info.n_out_rows)):
-                return True
-        return False
+        none = [sum(col) for col in zip(*(nr for nr, _ in self.stats()))]
+        return any(k == self.n_rows for k in none)
 
     def columns(self, part) -> List[Column]:
         return [part.column(c) for c in range(len(self.types))]
@@ -143,6 +151,8 @@ class DeviceRows:
         return None if any(c is None for c in chunks) else chunks
 
     def free(self):
+        if not self.owned:
+            return
         for p in self.parts:
             p.free()
         self.parts = []
@@ -165,6 +175,156 @@ class DeviceSource(Source):
 
     def to_host_source(self) -> Source:
         return self.ctx._source_from_rows(self.rows.rows(), self.names)
+
+
+class _CachedPart:
+    """One block of a cached dataset as a part of DeviceRows. It reads like a stage result; a consumer that takes it as a block gets
+    a view (as_block), so that freeing its input leaves the cache intact."""
+
+    def __init__(self, block, types: List[int]):
+        self.block, self.types, self.device = block, list(types), block.device
+        n = int(block.n_rows)
+        nb = block.column_bytes()
+        self.info = _PartInfo(n, [nb[c] - (n + 1) * 4 if t == T_STR else 0 for c, t in enumerate(self.types)])
+
+    def as_block(self, n_cols: Optional[int] = None):
+        return self.block.view()
+
+    def column(self, c: int) -> Column:
+        return self.block.column(c, self.types[c])
+
+    def validity(self, c: int):
+        return self.block.validity(c)
+
+    def free(self):
+        pass
+
+
+class _PartInfo:
+    def __init__(self, n_out_rows: int, out_str_bytes: List[int]):
+        self.n_out_rows, self.out_str_bytes = n_out_rows, out_str_bytes
+
+
+class CacheSource(DeviceSource):
+    """Input of a plan that cache() keeps on the device: blocks of tuplex.gpu.blockRows rows (the host source's cut), typed as
+    Context._source_from_rows types the same rows, owned by this source and freed when the last dataset that refers to it goes.
+    Every read borrows them (DeviceRows with borrowed parts)."""
+
+    def __init__(self, ctx, blocks: list, names: List[Optional[str]], types: List[int], option_cols: List[int]):
+        super().__init__(ctx, DeviceRows([_CachedPart(b, types) for b in blocks], names, types, owned=False))
+        self._option_cols = list(option_cols)
+        self.nbytes = sum(sum(b.column_bytes()) for b in blocks) + len(option_cols) * sum((int(b.n_rows) + 31) // 32 * 4 for b in blocks)
+        with _metrics_lock:
+            ctx.metrics.cache_rows += self.n_rows
+            ctx.metrics.cache_bytes += self.nbytes
+        weakref.finalize(self, _free_cache, list(blocks), ctx.metrics, self.nbytes)
+
+    @property
+    def option_cols(self) -> List[int]:
+        return list(self._option_cols)
+
+
+def _free_cache(blocks: list, metrics, nbytes: int):
+    for b in blocks:
+        b.free()
+    with _metrics_lock:
+        metrics.cache_bytes -= nbytes
+
+
+def _cache_flags(types: Sequence[int], none_rows: Sequence[int], invalid_utf8: Sequence[int], n_rows: int) -> List[Tuple[int, int, bool]]:
+    """(tplx_concat_flags, cached type, holds None) per column of n_rows > 0 rows: Context._source_from_rows's typing restated
+    from counts. A column without None is plain T (its bitmap is dropped), one with some None is Option[T], one that is None in
+    every row is i64 placeholders with a clear bitmap, whatever the stage's type was. Strings that are not valid UTF-8 are
+    rewritten as decode("utf-8", "replace") gives them."""
+    out = []
+    for t, k, bad in zip(types, none_rows, invalid_utf8):
+        utf8 = backend.CONCAT_UTF8 if t == T_STR and bad else 0
+        if k == n_rows:
+            out.append((backend.CONCAT_ALL_NONE, T_I64, True))
+        elif k == 0:
+            out.append((backend.CONCAT_DROP_VALID | utf8, t, False))
+        else:
+            out.append((utf8, t, True))
+    return out
+
+
+def _cache_plan(part_rows: Sequence[int], block_rows: int) -> List[List[Tuple[int, int, int]]]:
+    """The pieces (part, first row, rows) of every cached block: rows [k * block_rows, (k + 1) * block_rows) of the parts' rows
+    in order, the cut _column_blocks makes over a host source of the same rows. Empty parts give no piece."""
+    blocks: List[List[Tuple[int, int, int]]] = []
+    cur: List[Tuple[int, int, int]] = []
+    fill = 0
+    for p, n in enumerate(part_rows):
+        r = 0
+        while r < n:
+            take = min(n - r, block_rows - fill)
+            cur.append((p, r, take))
+            r += take
+            fill += take
+            if fill == block_rows:
+                blocks.append(cur)
+                cur, fill = [], 0
+    if cur:
+        blocks.append(cur)
+    return blocks
+
+
+def _device_cache(ctx, rows: DeviceRows, names) -> Tuple[Optional[DataSet], Optional[list]]:
+    """cache() of rows that a stage or join left on the device (at least one row): per-part statistics, column flags, then one
+    typed concatenation per output block, each consumed part freed as soon as its rows are copied (the peak is the data plus one
+    block). (dataset over a CacheSource, None); or, when the device runs out of memory, (None, the Python rows) with what was built
+    freed, for the host path."""
+    ncols = len(rows.types)
+    stats = rows.stats()
+    none = [sum(col) for col in zip(*(nr for nr, _ in stats))]
+    bad = [sum(col) for col in zip(*(iv for _, iv in stats))]
+    flags = _cache_flags(rows.types, none, bad, rows.n_rows)
+    sizes = [int(p.info.n_out_rows) for p in rows.parts]
+    plan = _cache_plan(sizes, ctx._block_rows)
+    views: Dict[int, Any] = {}
+    built: list = []
+    start = [0] * len(sizes)  # rows of each part already in built blocks
+    freed = 0                 # parts [0, freed) are released
+
+    def release(upto: int):
+        nonlocal freed
+        for p in range(freed, upto):
+            v = views.pop(p, None)
+            if v is not None:
+                v.free()
+            if rows.owned:
+                rows.parts[p].free()
+        freed = max(freed, upto)
+
+    try:
+        for pieces in plan:
+            for p, _, _ in pieces:
+                if p not in views:
+                    views[p] = rows.parts[p].as_block(ncols)
+            built.append(backend.Block.concat_pieces([(views[p], f, n) for p, f, n in pieces], [f for f, _, _ in flags]))
+            for p, f, n in pieces:
+                start[p] = f + n
+            p, f, n = pieces[-1]
+            release(p + 1 if f + n == sizes[p] else p)
+    except backend.GpuBackendError as e:
+        if e.code != backend.E_NOMEM:
+            raise
+        ctx._log(f"cache() falls back to host rows: {e}")
+        vals: List[list] = [[] for _ in range(ncols)]
+        for b in built:
+            for c, (_, t, _) in enumerate(flags):
+                vals[c].extend(b.column(c, t).to_values())
+            b.free()
+        for p in range(freed, len(sizes)):
+            for c, col in enumerate(rows.columns(rows.parts[p])):
+                vals[c].extend(col.to_values()[start[p]:])
+        release(len(sizes))
+        rows.free()
+        return None, (vals[0] if ncols == 1 else list(zip(*vals)))
+    release(len(sizes))
+    rows.free()
+    src = CacheSource(ctx, built, names, [t for _, t, _ in flags], [c for c, (_, _, opt) in enumerate(flags) if opt])
+    return DataSet(ctx, src), None
 
 
 def _handoff_ok(ctx) -> bool:
@@ -309,7 +469,21 @@ class DataSet:
         return self._with(Op("unique"))
 
     def cache(self, store_specialized=True):
-        rows, names = self._execute()
+        """Run the pipeline and keep its rows for every later action and branch. On one device, with None kept in the normal case,
+        rows that a stage or join leaves on the device stay there as owned blocks (a CacheSource), typed, cut and encoded exactly as
+        the host source of the same rows would be; otherwise (and for zero rows, fallback rows, aggregate endpoints) the rows come
+        to the host and become a host source. `store_specialized` is accepted for the reference's signature."""
+        src = self._source
+        if isinstance(src, CacheSource) and not self._ops and self._join is None and self._parent is None:
+            return DataSet(self._ctx, src)
+        rows, names = self._execute(handoff=_handoff_ok(self._ctx))
+        if isinstance(rows, DeviceRows):
+            if rows.n_rows:
+                ds, rows = _device_cache(self._ctx, rows, names)
+                if ds is not None:
+                    return ds
+            else:
+                rows = rows.rows()
         return self._ctx._dataset_from_rows(rows, names)
 
     # ---- actions ------------------------------------------------------------------------------------
@@ -415,7 +589,7 @@ class DataSet:
     def _names_after_map(self, op, names):
         """Compile (never run) the operator chain up to `op` to learn the shape its map() returns; UDFs outside the GPU op set
         fall back to reading the UDF's return expression."""
-        if self._parent is None and self._source is not None and len(self._source.cols) == len(names):
+        if self._parent is None and self._source is not None and len(self._source.col_types) == len(names):
             try:
                 return list(_compile_row_ops(self._source, self._ops[:self._ops.index(op) + 1]).names)
             except Exception:  # noqa: BLE001 — UnsupportedUDF or a UDF the front end cannot read
@@ -428,6 +602,8 @@ class DataSet:
         `handoff` (the consumer is a join) a last row stage may instead return its results on the device, as a DeviceRows."""
         src = self._source
         self._last_exceptions = Counter()
+        if handoff and isinstance(src, CacheSource) and not self._ops and self._parent is None:
+            return src.rows, list(src.names)  # the cache's blocks, borrowed: no stage needs to copy them
         if self._join is not None:
             rows, names = _run_join(self._ctx, self._join, self._last_exceptions, handoff or csv_sink is not None or bool(self._ops))
             if isinstance(rows, DeviceRows):
