@@ -78,7 +78,9 @@ typedef struct tplx_result_info {
     uint64_t h2d_bytes;      /* run_host: bytes of input explicitly copied host->device */
     uint32_t specialised_launches; /* of kernel_launches: kernels the stage specialiser compiled for this stage (csrc/jit.inl);
                                       0 = the interpreting kernels ran */
-    uint32_t pad_info;
+    uint32_t lane;                 /* execution lane of the GPU that ran the block: 0 = the primary lane, 1 = the second lane a
+                                      concurrent caller takes while the primary one is busy; results not made by a stage run
+                                      (hash_finish, joins, merges, ...) report 0 */
 } tplx_result_info;
 
 /* ---- process / devices ------------------------------------------------------------------ */

@@ -40,7 +40,7 @@ class CResultInfo(ct.Structure):
     _fields_ = [("n_in_rows", ct.c_uint64), ("n_out_rows", ct.c_uint64), ("n_exceptions", ct.c_uint64),
                 ("out_str_bytes", ct.c_uint64 * MAX_COLS), ("kernel_ms", ct.c_double), ("total_ms", ct.c_double),
                 ("kernel_launches", ct.c_uint32), ("zero_copy_cols", ct.c_uint32), ("h2d_bytes", ct.c_uint64),
-                ("specialised_launches", ct.c_uint32), ("pad_info", ct.c_uint32)]
+                ("specialised_launches", ct.c_uint32), ("lane", ct.c_uint32)]
 
 
 class CCsvDesc(ct.Structure):

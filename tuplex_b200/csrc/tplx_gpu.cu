@@ -13,6 +13,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <atomic>
 #include <chrono>
 #include <memory>
 #include <mutex>
@@ -413,6 +414,7 @@ struct StageDev {
     Device *dev = nullptr;
     DInstr *prog = nullptr;  // pre-decoded program
     DInstr *prog_vec[2] = {nullptr, nullptr};  // the same for the vector kernel (slot stride of T = 1024 / 2048 rows), built on demand
+                                               // (written and read under tplx_stage::mu)
     uint8_t *cpool = nullptr;
     int64_t *opids = nullptr;
     HashTable *ht = nullptr;  // HASH endpoint
@@ -433,12 +435,14 @@ struct tplx_stage {
     bool materialises = false;
     uint32_t n_str_out = 0;
     std::vector<StageDev> devs;
+    // Run-time state that later blocks are sized from. Blocks of one stage run concurrently on the GPU's execution lanes, so a
+    // field may be written by one caller while another reads it: relaxed atomics (any recent value is a valid estimate).
     // adaptive output capacities learnt from earlier blocks (bytes per input row per str out col)
-    std::vector<double> est_bytes_per_row;
-    double est_exc_per_row = 0.0;
+    std::atomic<double> est_bytes_per_row[TPLX_MAX_COLS];
+    std::atomic<double> est_exc_per_row{0.0};
     tplx_stage *prefilter = nullptr;  // nested selective stage (row index output), may be null
-    bool prefilter_enabled = true;    // switched off at run time when it turns out not to be selective
-    double est_surv_ratio = -1.0;     // survivors / rows of the last block (prefilter stage): sizes the next block's dense launch
+    std::atomic<bool> prefilter_enabled{true};  // switched off at run time when it turns out not to be selective
+    std::atomic<double> est_surv_ratio{-1.0};   // survivors / rows of the last block (prefilter stage): sizes the next block's dense launch
     uint32_t hidden = 0;              // trailing executor-internal output columns
     bool vec_ok = false;              // fixed-width values and vector-VM ops only: eligible for K1v (vecvm.cuh)
     VecPlan vplan;                    // K1v micro-op program (accumulator chains, fused compare/filter), built when vec_ok
@@ -448,9 +452,10 @@ struct tplx_stage {
     // stage specialiser (jit.inl): live-out slots (the compact register file of the specialised kernels), one binary per kernel kind
     jit::LiveOut jit_live;
     std::map<int, std::shared_ptr<jit::Binary>> jit_bin;
-    bool jit_hot = false;             // a block large enough to pay for the compile has been seen
+    std::atomic<bool> jit_hot{false};  // a block large enough to pay for the compile has been seen
     std::mutex mu;
 };
+static constexpr std::memory_order relaxed = std::memory_order_relaxed;
 
 static size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
@@ -643,7 +648,7 @@ extern "C" int32_t tplx_gpu_stage_create(const void *desc, uint64_t desc_bytes, 
     if (h.endpoint > TPLX_EP_HASH) return bad("stage descriptor: unknown endpoint");
     if (h.endpoint == TPLX_EP_AGGREGATE && h.n_accs == 0) return bad("aggregate endpoint without accumulators");
     if (h.endpoint == TPLX_EP_HASH && (h.n_keys == 0 || h.n_keys > h.n_out_cols)) return bad("hash endpoint without key columns");
-    s->est_bytes_per_row.assign(h.n_out_cols, -1.0);
+    for (auto &e : s->est_bytes_per_row) e.store(-1.0, relaxed);
     // K1v eligibility: no string value anywhere and only operations the vector VM implements
     s->vec_ok = !s->has_str && h.endpoint == TPLX_EP_MEMORY && h.n_instr > 0;
     for (const tplx_instr &in : s->instrs) {
@@ -727,8 +732,8 @@ static int jit_minb(const tplx_stage *s, int kind) {
 static bool jit_wanted(tplx_stage *s, uint64_t block_rows) {
     const int m = jit::mode();
     if (m <= 0 || s->instrs.empty()) return false;
-    if (m >= 2 || block_rows >= jit::min_rows()) s->jit_hot = true;
-    return s->jit_hot;
+    if (m >= 2 || block_rows >= jit::min_rows()) s->jit_hot.store(true, relaxed);
+    return s->jit_hot.load(relaxed);
 }
 // nullptr: not available (NVRTC / driver entry points missing, compile or load failed) — the interpreting kernel runs instead
 static jit::Loaded *jit_get(tplx_stage *s, StageDev *sd, int kind, int minb) {
@@ -1019,6 +1024,7 @@ struct tplx_result {
     uint32_t zero_copy_cols = 0;  // input columns read in place from page-locked host memory
     uint32_t launches = 0;
     uint32_t jit_launches = 0;  // of those: kernels produced by the stage specialiser
+    uint32_t lane = 0;          // execution lane that ran the block (0 = the device's primary lane, 1 = its `alt`)
     bool owns_block = false;
     tplx_block *owned_block = nullptr;
     tplx_block *expanded_block = nullptr;  // the input block plus the `is None` companions of its Option[T] columns (tplx_gpu_stage_run)
@@ -1208,9 +1214,11 @@ static int32_t stage_run_impl(tplx_stage *s, const tplx_block *b, int64_t first_
     // several execution lanes per GPU: a concurrent caller does not wait for the first one's kernels, it takes the next
     // free lane (hash stages keep to the primary lane: one table per device)
     std::unique_lock<std::mutex> lk(d->mu, std::try_to_lock);
+    uint32_t lane = 0;
     while (!lk.owns_lock()) {
         if (s->hdr.endpoint != TPLX_EP_HASH && d->alt) {
             d = d->alt;
+            ++lane;
             lk = d->alt ? std::unique_lock<std::mutex>(d->mu, std::try_to_lock) : std::unique_lock<std::mutex>(d->mu);
         } else {
             lk = std::unique_lock<std::mutex>(d->mu);
@@ -1222,6 +1230,7 @@ static int32_t stage_run_impl(tplx_stage *s, const tplx_block *b, int64_t first_
     if (rc) return rc;
     tplx_result *r = new tplx_result();
     r->dev = d;
+    r->lane = lane;
     r->stage = s;
     r->block = b;
     r->n_in = b->n_rows;
@@ -1246,7 +1255,7 @@ static int32_t stage_run_impl(tplx_stage *s, const tplx_block *b, int64_t first_
             else if (lazy_read_early)
                 rc = fail(TPLX_E_BADARG, "stage_run: a column parsed with col_lazy is read by the stage's prefilter; parse it eagerly");
             else
-                rc = (s->prefilter && (s->prefilter_enabled || lazy)) ? run_rows_prefiltered(s, sd, b, first_row_no, r)
+                rc = (s->prefilter && (s->prefilter_enabled.load(relaxed) || lazy)) ? run_rows_prefiltered(s, sd, b, first_row_no, r)
                                                                         : run_rows(s, sd, b, first_row_no, r, nullptr, 0);
             break;
         }
@@ -1280,7 +1289,7 @@ extern "C" int32_t tplx_gpu_stage_run_host(tplx_stage *s, int32_t device, const 
     int32_t rc = TPLX_OK;
     uint64_t h2d = 0;
     uint32_t zc = 0;
-    if (s && s->prefilter && s->prefilter_enabled && s->hdr.endpoint == TPLX_EP_MEMORY && cols && n_cols == s->in_types.size() && !s->n_companions) {
+    if (s && s->prefilter && s->prefilter_enabled.load(relaxed) && s->hdr.endpoint == TPLX_EP_MEMORY && cols && n_cols == s->in_types.size() && !s->n_companions) {
         // Late materialisation across PCIe: only the columns the prefilter reads are copied to HBM. The other
         // columns are needed for surviving rows only; when they lie in page-locked host memory the dense launch
         // reads exactly those rows through the mapped address (zero-copy), otherwise they are copied like before.
@@ -1446,19 +1455,21 @@ static int32_t run_rows_vec(tplx_stage *s, StageDev *sd, const tplx_block *b, in
     if (!Jsel) return TPLX_E_UNSUPPORTED;
     const uint32_t smem = L.total;
     const int ji = Jsel == 4 ? 1 : 0;
-    if (!jf && !sd->prog_vec[ji]) {
+    DInstr *prog_vec = nullptr;
+    {  // built by the first block that needs it; both lanes may get here at once, so it is read under the lock too
         std::lock_guard<std::mutex> lk(s->mu);
-        if (!sd->prog_vec[ji]) {
+        if (!jf && !sd->prog_vec[ji]) {
             std::vector<VInstr> dec = vec_encode(s->vplan, T, L.regs_off);
             VInstr *p = nullptr;
             CU(cudaMalloc(&p, std::max<size_t>(dec.size() * sizeof(VInstr), 16)));
             CU(cudaMemcpy(p, dec.data(), dec.size() * sizeof(VInstr), cudaMemcpyHostToDevice));
             sd->prog_vec[ji] = reinterpret_cast<DInstr *>(p);
         }
+        prog_vec = sd->prog_vec[ji];
     }
     KParams P;
     fill_common(P, s, sd, b, L, 2 * Jsel);
-    P.prog = sd->prog_vec[ji];
+    P.prog = prog_vec;
     P.n_instr = jf ? 0u : (uint32_t)n_uops;
     P.n_slots = jf ? (uint32_t)s->jit_live.slots.size() : ns;
 
@@ -1510,7 +1521,7 @@ static int32_t run_rows_vec(tplx_stage *s, StageDev *sd, const tplx_block *b, in
         if (rc) return rc;
     }
     P.cap_rows = n;
-    uint64_t cap_exc = std::max<uint64_t>(4096, (uint64_t)(s->est_exc_per_row * 1.5 * (double)n) + n / 64);
+    uint64_t cap_exc = std::max<uint64_t>(4096, (uint64_t)(s->est_exc_per_row.load(relaxed) * 1.5 * (double)n) + n / 64);
     for (int attempt = 0; attempt < 2; ++attempt) {
         P.cap_exc = cap_exc;
         rc = dalloc(r, &P.exc, cap_exc);
@@ -1530,7 +1541,7 @@ static int32_t run_rows_vec(tplx_stage *s, StageDev *sd, const tplx_block *b, in
         CU(cudaStreamSynchronize(d->stream));
         r->n_out = h_tot[0];
         r->n_exc = h_tot[1];
-        s->est_exc_per_row = (double)r->n_exc / (double)n;
+        s->est_exc_per_row.store((double)r->n_exc / (double)n, relaxed);
         if (h_cnt[1] == 0) break;
         if (attempt == 1) return fail(TPLX_E_OVERFLOW, "exception capacity retry failed");
         cap_exc = r->n_exc + 16;
@@ -1646,11 +1657,11 @@ static int32_t run_rows(tplx_stage *s, StageDev *sd, const tplx_block *b, int64_
     std::vector<uint64_t> cap_bytes(s->out_cols.size(), 0);
     for (size_t c = 0; c < s->out_cols.size(); ++c) {
         if (s->out_cols[c].type != TPLX_T_STR) continue;
-        double est = s->est_bytes_per_row[c];
+        const double est = s->est_bytes_per_row[c].load(relaxed);
         uint64_t cap = est >= 0 ? (uint64_t)(est * 1.25 * (double)n) + (1u << 16) : in_str_bytes / 8 + n + (1u << 20);
         cap_bytes[c] = std::min<uint64_t>(cap, 0xFFFFFFFFull);
     }
-    uint64_t cap_exc = std::max<uint64_t>(4096, (uint64_t)(s->est_exc_per_row * 1.5 * (double)n) + n / 64);
+    uint64_t cap_exc = std::max<uint64_t>(4096, (uint64_t)(s->est_exc_per_row.load(relaxed) * 1.5 * (double)n) + n / 64);
     uint64_t cap_rows = n;
 
     uint64_t *tile_state = nullptr, *totals = nullptr;
@@ -1719,9 +1730,9 @@ static int32_t run_rows(tplx_stage *s, StageDev *sd, const tplx_block *b, int64_
         for (size_t c = 0; c < s->out_cols.size(); ++c)
             if (s->out_cols[c].type == TPLX_T_STR) {
                 r->str_bytes[c] = h_tot[2 + si++];
-                s->est_bytes_per_row[c] = (double)r->str_bytes[c] / (double)n_act;
+                s->est_bytes_per_row[c].store((double)r->str_bytes[c] / (double)n_act, relaxed);
             }
-        s->est_exc_per_row = (double)r->n_exc / (double)n_act;
+        s->est_exc_per_row.store((double)r->n_exc / (double)n_act, relaxed);
         if (h_cnt[1] & 8u) return TPLX_INTERNAL_RETRY;  // more survivors than the estimate everything was sized for
         if (h_cnt[1] == 0) break;
         if (attempt == 2) return fail(TPLX_E_OVERFLOW, "output capacity retry failed");
@@ -1825,7 +1836,7 @@ static int32_t run_mask(tplx_stage *ps, StageDev *psd, const tplx_block *b, tplx
     CU(cudaGetLastError());
     if (totals_dev) *totals_dev = totals;
     if (no_wait) {
-        const uint64_t cap_exc = std::max<uint64_t>(4096, (uint64_t)(ps->est_exc_per_row * 1.5 * (double)n) + n / 64);
+        const uint64_t cap_exc = std::max<uint64_t>(4096, (uint64_t)(ps->est_exc_per_row.load(relaxed) * 1.5 * (double)n) + n / 64);
         if (cap_exc_out) *cap_exc_out = cap_exc;
         rc = dalloc(ra, &ra->out[0].data, n);  // worst case: every row survives
         if (rc) return rc;
@@ -1890,7 +1901,8 @@ static int32_t run_rows_prefiltered(tplx_stage *s, StageDev *sd, const tplx_bloc
     // Steady state without a host round trip between the two launches: once a block has shown the selectivity, the dense launch of
     // the next block is sized from it (x1.3 + slack) and reads the real survivor count on the device; the host synchronises once,
     // at the end. (Blocks with late columns in host memory size their gather from the exact count and keep the round trip.)
-    const bool no_wait = !any_mapped && ps->est_surv_ratio >= 0.0 && b->n_rows > 0 && !(getenv("TPLX_SYNC_PREFILTER") && atoi(getenv("TPLX_SYNC_PREFILTER")));
+    const double est_surv = ps->est_surv_ratio.load(relaxed);  // read once: the check and the sizing below see the same value
+    const bool no_wait = !any_mapped && est_surv >= 0.0 && b->n_rows > 0 && !(getenv("TPLX_SYNC_PREFILTER") && atoi(getenv("TPLX_SYNC_PREFILTER")));
     uint64_t *totals_dev = nullptr, cap_exc_a = 0;
     rc = run_mask(ps, psd, b, &ra, no_wait, &totals_dev, &cap_exc_a);
     if (rc) { drop_ra(); return rc; }
@@ -1899,13 +1911,13 @@ static int32_t run_rows_prefiltered(tplx_stage *s, StageDev *sd, const tplx_bloc
     ra.evk0 = ra.evk1 = nullptr;
     float msa = 0;
     if (no_wait) {
-        const uint64_t cap = std::min<uint64_t>(b->n_rows, (uint64_t)(ps->est_surv_ratio * 1.3 * (double)b->n_rows) + 65536);
+        const uint64_t cap = std::min<uint64_t>(b->n_rows, (uint64_t)(est_surv * 1.3 * (double)b->n_rows) + 65536);
         rc = run_rows(s, sd, b, first_row_no, r, ra.out[0].data, cap, nullptr, totals_dev);  // synchronises the stream at its end
         if (rc != TPLX_OK && rc != TPLX_INTERNAL_RETRY) { drop_ra(); return rc; }
         ra.n_out = d->pinned[0];
         ra.n_exc = d->pinned[1];
-        ps->est_surv_ratio = (double)ra.n_out / (double)b->n_rows;
-        ps->est_exc_per_row = (double)ra.n_exc / (double)b->n_rows;
+        ps->est_surv_ratio.store((double)ra.n_out / (double)b->n_rows, relaxed);
+        ps->est_exc_per_row.store((double)ra.n_exc / (double)b->n_rows, relaxed);
         if (ra.n_exc > cap_exc_a) {  // more prefilter exceptions than estimated: expand them again with the exact capacity
             int32_t rc2 = dalloc(&ra, &ra.exc, ra.n_exc);
             if (rc2) { drop_ra(); return rc2; }
@@ -1928,9 +1940,12 @@ static int32_t run_rows_prefiltered(tplx_stage *s, StageDev *sd, const tplx_bloc
     }
     const uint64_t n_surv = ra.n_out;
     if (!no_wait) {
-        if (b->n_rows) { ps->est_surv_ratio = (double)n_surv / (double)b->n_rows; ps->est_exc_per_row = (double)ra.n_exc / (double)b->n_rows; }
+        if (b->n_rows) {
+            ps->est_surv_ratio.store((double)n_surv / (double)b->n_rows, relaxed);
+            ps->est_exc_per_row.store((double)ra.n_exc / (double)b->n_rows, relaxed);
+        }
     }
-    if (b->n_rows >= (1u << 16) && n_surv * 2 > b->n_rows) s->prefilter_enabled = false;  // not selective: stop using it
+    if (b->n_rows >= (1u << 16) && n_surv * 2 > b->n_rows) s->prefilter_enabled.store(false, relaxed);  // not selective: stop using it
     // late columns that still live in host memory: bring over the surviving rows only (gather.cuh)
     std::vector<ColIn> dense_cols;
     float msg = 0;
@@ -2192,7 +2207,7 @@ static int32_t run_agg(tplx_stage *s, StageDev *sd, const tplx_block *b, tplx_re
     int32_t rc = ensure_scratch(d, (size_t)grid * NT * P.scratch_per_thread);
     if (rc) return rc;
     P.scratch = d->scratch;
-    uint64_t cap_exc = std::max<uint64_t>(4096, (uint64_t)(s->est_exc_per_row * 1.5 * (double)n) + n / 64);
+    uint64_t cap_exc = std::max<uint64_t>(4096, (uint64_t)(s->est_exc_per_row.load(relaxed) * 1.5 * (double)n) + n / 64);
     KParams *dP = nullptr;
     uint32_t *counters = nullptr;
     rc = dalloc(r, &P.tile_partials, (size_t)std::max<uint32_t>(P.n_tiles, 1) * P.n_accs);
@@ -2234,7 +2249,7 @@ static int32_t run_agg(tplx_stage *s, StageDev *sd, const tplx_block *b, tplx_re
         CU(cudaMemcpyAsync(h_cnt, counters, 16, cudaMemcpyDeviceToHost, d->stream));
         CU(cudaStreamSynchronize(d->stream));
         r->n_exc = h_cnt[2];
-        if (n) s->est_exc_per_row = (double)r->n_exc / (double)n;
+        if (n) s->est_exc_per_row.store((double)r->n_exc / (double)n, relaxed);
         if (!(h_cnt[1] & 4u)) break;
         cap_exc = r->n_exc + 16;
         if (attempt == 1) return fail(TPLX_E_OVERFLOW, "exception capacity retry failed");
@@ -2280,6 +2295,7 @@ extern "C" int32_t tplx_gpu_result_info(tplx_result *r, tplx_result_info *info) 
     info->total_ms = r->total_ms;
     info->kernel_launches = r->launches;
     info->specialised_launches = r->jit_launches;
+    info->lane = r->lane;
     info->zero_copy_cols = r->zero_copy_cols;
     info->h2d_bytes = r->h2d_bytes;
     return TPLX_OK;
