@@ -1,5 +1,7 @@
-// gather.cuh — late materialisation of "late" columns for the rows a prefilter stage let through.
+// gather.cuh — device columns built from selected rows of other columns: the late materialisation below, and the gather by row
+// selector of join and merge outputs at the end of the file.
 //
+// Late materialisation of "late" columns for the rows a prefilter stage let through.
 // When the inputs of tplx_gpu_stage_run_host lie in page-locked host memory, only the columns the prefilter
 // reads are copied to HBM up front. The remaining columns are needed for the surviving rows only: these kernels
 // read exactly those rows through the mapped host address (many independent, coalesced reads in flight, so the
@@ -74,6 +76,85 @@ __global__ void gather_pass2(uint64_t n, const GatherCols *__restrict__ G, const
         }
         for (uint32_t k = lane; k < len; k += 32) dst[k] = src[k];
     }
+}
+
+// ---- gather by row selector: output columns built from rows of up to two device columns (K8 join outputs, K9 merge) ----------
+// One u32 selector per output row. SEL_NONE: no source row (value 0, length 0, validity bit clear). Otherwise the row is
+// s & ~b_bit of source B when s & b_bit, else of source A. A source without a bitmap gives set bits. Sources are read with __ldg:
+// a pointer picked from a struct is not known to be global memory, and a plain load would not take the read-only path.
+constexpr uint32_t SEL_NONE = 0xFFFFFFFFu;
+constexpr uint32_t SEL_NT = 256;
+constexpr uint32_t SEL_STR_LANES = 8;  // lanes that copy one output string
+
+struct SelSrc {
+    const void *data;         // 8-byte values, or string bytes
+    const uint32_t *offsets;  // strings: n + 1 offsets
+    const uint32_t *valid;    // validity bitmap, or nullptr
+};
+
+__device__ __forceinline__ SelSrc sel_src(uint32_t s, uint32_t b_bit, const SelSrc &a, const SelSrc &b, uint32_t *row) {
+    *row = s & ~b_bit;
+    return (s & b_bit) ? b : a;
+}
+
+__global__ void __launch_bounds__(SEL_NT) sel_gather_fixed_kernel(SelSrc a, SelSrc b, uint32_t b_bit, const uint32_t *__restrict__ sel, uint64_t n,
+                                                                   uint64_t *__restrict__ dst) {
+    const uint64_t i = (uint64_t)blockIdx.x * SEL_NT + threadIdx.x;
+    if (i >= n) return;
+    const uint32_t s = sel[i];
+    if (s == SEL_NONE) { dst[i] = 0; return; }
+    uint32_t r;
+    const SelSrc src = sel_src(s, b_bit, a, b, &r);
+    dst[i] = __ldg(static_cast<const uint64_t *>(src.data) + r);
+}
+
+// one validity word per warp
+__global__ void __launch_bounds__(SEL_NT) sel_gather_valid_kernel(SelSrc a, SelSrc b, uint32_t b_bit, const uint32_t *__restrict__ sel, uint64_t n,
+                                                                   uint32_t *__restrict__ dst_words) {
+    const uint64_t i = (uint64_t)blockIdx.x * SEL_NT + threadIdx.x;
+    bool ok = false;
+    if (i < n) {
+        const uint32_t s = sel[i];
+        if (s != SEL_NONE) {
+            uint32_t r;
+            const uint32_t *v = sel_src(s, b_bit, a, b, &r).valid;
+            ok = !v || ((__ldg(v + (r >> 5)) >> (r & 31)) & 1u);
+        }
+    }
+    const uint32_t w = __ballot_sync(0xFFFFFFFFu, ok);
+    if ((threadIdx.x & 31) == 0 && (i >> 5) < ((n + 31) >> 5)) dst_words[i >> 5] = w;
+}
+
+// strings: lengths (then an exclusive scan in place), then the bytes
+__global__ void __launch_bounds__(SEL_NT) sel_str_len_kernel(SelSrc a, SelSrc b, uint32_t b_bit, const uint32_t *__restrict__ sel, uint64_t n,
+                                                              uint64_t *__restrict__ lens) {
+    const uint64_t i = (uint64_t)blockIdx.x * SEL_NT + threadIdx.x;
+    if (i >= n) return;
+    const uint32_t s = sel[i];
+    if (s == SEL_NONE) { lens[i] = 0; return; }
+    uint32_t r;
+    const uint32_t *o = sel_src(s, b_bit, a, b, &r).offsets;
+    lens[i] = __ldg(o + r + 1) - __ldg(o + r);
+}
+
+__global__ void __launch_bounds__(SEL_NT) sel_str_copy_kernel(SelSrc a, SelSrc b, uint32_t b_bit, const uint32_t *__restrict__ sel, uint64_t n,
+                                                               const uint64_t *__restrict__ pos, uint32_t *__restrict__ dst_off, uint8_t *__restrict__ dst) {
+    // SEL_STR_LANES lanes per output row: the strings of these paths are short (codes, names: 8 B in the bench's join table), so a
+    // whole warp per row would leave most lanes idle; 8 lanes keep one byte per lane and row in flight
+    const uint64_t t = (uint64_t)blockIdx.x * SEL_NT + threadIdx.x;
+    const uint64_t i = t / SEL_STR_LANES;
+    const uint32_t sub = (uint32_t)(t % SEL_STR_LANES);
+    if (i > n) return;
+    const uint64_t d0 = pos[i];
+    if (sub == 0) dst_off[i] = (uint32_t)d0;  // entry n = total
+    if (i == n) return;
+    const uint32_t s = sel[i];
+    if (s == SEL_NONE) return;
+    uint32_t r;
+    const SelSrc src = sel_src(s, b_bit, a, b, &r);
+    const uint8_t *bytes = static_cast<const uint8_t *>(src.data);
+    const uint32_t s0 = __ldg(src.offsets + r), len = __ldg(src.offsets + r + 1) - s0;
+    for (uint32_t k = sub; k < len; k += SEL_STR_LANES) dst[d0 + k] = __ldg(bytes + s0 + k);
 }
 
 }  // namespace tplx

@@ -21,7 +21,7 @@
 //                   than one row is put in order: thread-per-group insertion sort, CTA-per-group counting rank for
 //                   groups above 32 rows).
 // Probe = two passes over the probe block (count, exclusive scan, emit) giving (probe row, build row) index pairs in the
-// output order above, then a columnar gather of every output column with validity bitmaps where a column is nullable.
+// output order above, then a columnar gather of every output column (gather.cuh) with validity bitmaps where a column is nullable.
 // The probe is HBM-latency work (one random slot + one random key read per probe row): 256-thread CTAs, grid sized to the
 // block, every lane independent; bucket loops of 32+ rows are taken by the whole warp.
 #pragma once
@@ -34,7 +34,6 @@ namespace tplx {
 constexpr uint32_t JOIN_NONE = 0xFFFFFFFFu;
 constexpr uint32_t JOIN_NT = 256;
 constexpr uint32_t JOIN_SMALL = 32;  // groups up to this size are ordered by one thread
-constexpr uint32_t JOIN_STR_LANES = 8;  // lanes that copy one output string
 
 struct JoinKey {            // a key column (build or probe side)
     const void *data;       // 8-byte values, or string bytes
@@ -226,53 +225,6 @@ __global__ void __launch_bounds__(JOIN_NT) join_probe_emit_kernel(JoinTableDev T
             out_build[rb + j] = T.rows[rs + j];
         }
     }
-}
-
-// ---- gather of the output columns -------------------------------------------------------------------------------------------
-// fixed width: dst[i] = src[idx[i]] (0 where idx is none)
-__global__ void __launch_bounds__(JOIN_NT) join_gather_fixed_kernel(const uint64_t *__restrict__ src, const uint32_t *__restrict__ idx, uint64_t n,
-                                                                    uint64_t *__restrict__ dst) {
-    const uint64_t i = (uint64_t)blockIdx.x * JOIN_NT + threadIdx.x;
-    if (i >= n) return;
-    const uint32_t r = idx[i];
-    dst[i] = r == JOIN_NONE ? 0ull : src[r];
-}
-// validity of an output column: one word per warp. bit = row has a source row and the source value is present
-__global__ void __launch_bounds__(JOIN_NT) join_gather_valid_kernel(const uint32_t *__restrict__ src_valid, const uint32_t *__restrict__ idx, uint64_t n,
-                                                                    uint32_t *__restrict__ dst_words) {
-    const uint64_t i = (uint64_t)blockIdx.x * JOIN_NT + threadIdx.x;
-    bool ok = false;
-    if (i < n) {
-        const uint32_t r = idx[i];
-        ok = r != JOIN_NONE && (!src_valid || ((src_valid[r >> 5] >> (r & 31)) & 1u));
-    }
-    const uint32_t w = __ballot_sync(0xFFFFFFFFu, ok);
-    if ((threadIdx.x & 31) == 0 && (i >> 5) < ((n + 31) >> 5)) dst_words[i >> 5] = w;
-}
-// strings: lengths (then an exclusive scan), then JOIN_STR_LANES lanes per output row copy the bytes
-__global__ void __launch_bounds__(JOIN_NT) join_str_len_kernel(const uint32_t *__restrict__ src_off, const uint32_t *__restrict__ idx, uint64_t n,
-                                                               uint64_t *__restrict__ lens) {
-    const uint64_t i = (uint64_t)blockIdx.x * JOIN_NT + threadIdx.x;
-    if (i >= n) return;
-    const uint32_t r = idx[i];
-    lens[i] = r == JOIN_NONE ? 0ull : (uint64_t)(src_off[r + 1] - src_off[r]);
-}
-__global__ void __launch_bounds__(JOIN_NT) join_str_copy_kernel(const uint8_t *__restrict__ src, const uint32_t *__restrict__ src_off,
-                                                                const uint32_t *__restrict__ idx, uint64_t n, const uint64_t *__restrict__ pos,
-                                                                uint32_t *__restrict__ dst_off, uint8_t *__restrict__ dst) {
-    // JOIN_STR_LANES lanes per output row: the strings of this path are short (codes, names: 8 B in the bench's table), so a whole
-    // warp per row would leave most lanes idle; 8 lanes keep one byte per lane and row in flight
-    const uint64_t t = (uint64_t)blockIdx.x * JOIN_NT + threadIdx.x;
-    const uint64_t i = t / JOIN_STR_LANES;
-    const uint32_t sub = (uint32_t)(t % JOIN_STR_LANES);
-    if (i > n) return;
-    const uint64_t d0 = pos[i];
-    if (sub == 0) dst_off[i] = (uint32_t)d0;  // entry n = total
-    if (i == n) return;
-    const uint32_t r = idx[i];
-    if (r == JOIN_NONE) return;
-    const uint32_t s0 = src_off[r], len = src_off[r + 1] - s0;
-    for (uint32_t k = sub; k < len; k += JOIN_STR_LANES) dst[d0 + k] = src[s0 + k];
 }
 
 }  // namespace tplx

@@ -6,13 +6,15 @@
 // task's output stream it occupied (TransformTask.cc:764,885), an unresolved one leaves its slot empty.
 // Closed form used here: exceptions sorted by row number r_0 < r_1 < ...; exception k had a_k = r_k - k normal rows before it. With the
 // resolved subset m = 0 .. n_res - 1 (ascending): normal row j lands at j + #{m : a_m <= j}, resolved row m at a_m + m. One kernel
-// writes the source selector of every output position, the gathers then move each column once (columnar, coalesced on the output side).
+// writes the source selector of every output position, the gathers by selector (gather.cuh) then move each column once (columnar, coalesced
+// on the output side).
 #pragma once
 #include <stdint.h>
 
 namespace tplx {
 
 constexpr uint32_t MERGE_B = 0x80000000u;  // selector flag: the row comes from the resolved block
+// a selector never equals SEL_NONE (gather.cuh): tplx_gpu_result_merge_resolved refuses n_norm + n_res >= 2^31 - 1
 
 // sel[n_norm + n_res]: j (normal row) or MERGE_B | m (resolved row)
 __global__ void __launch_bounds__(256) merge_select_kernel(const uint64_t *__restrict__ a_res, uint64_t n_res, uint64_t n_norm, uint32_t *__restrict__ sel) {
@@ -29,55 +31,6 @@ __global__ void __launch_bounds__(256) merge_select_kernel(const uint64_t *__res
         const uint64_t m = i - n_norm;
         sel[a_res[m] + m] = MERGE_B | (uint32_t)m;
     }
-}
-
-__global__ void __launch_bounds__(256) merge_fixed_kernel(const uint64_t *__restrict__ a, const uint64_t *__restrict__ b, const uint32_t *__restrict__ sel,
-                                                          uint64_t n, uint64_t *__restrict__ dst) {
-    const uint64_t i = (uint64_t)blockIdx.x * 256 + threadIdx.x;
-    if (i >= n) return;
-    const uint32_t s = sel[i];
-    dst[i] = (s & MERGE_B) ? b[s & ~MERGE_B] : a[s];
-}
-
-__global__ void __launch_bounds__(256) merge_valid_kernel(const uint32_t *__restrict__ va, const uint32_t *__restrict__ vb, const uint32_t *__restrict__ sel,
-                                                          uint64_t n, uint32_t *__restrict__ words) {
-    const uint64_t i = (uint64_t)blockIdx.x * 256 + threadIdx.x;
-    bool ok = false;
-    if (i < n) {
-        const uint32_t s = sel[i], r = s & ~MERGE_B;
-        const uint32_t *v = (s & MERGE_B) ? vb : va;
-        ok = !v || ((v[r >> 5] >> (r & 31)) & 1u);
-    }
-    const uint32_t w = __ballot_sync(0xFFFFFFFFu, ok);
-    if ((threadIdx.x & 31) == 0 && (i >> 5) < ((n + 31) >> 5)) words[i >> 5] = w;
-}
-
-__global__ void __launch_bounds__(256) merge_str_len_kernel(const uint32_t *__restrict__ oa, const uint32_t *__restrict__ ob, const uint32_t *__restrict__ sel,
-                                                            uint64_t n, uint64_t *__restrict__ lens) {
-    const uint64_t i = (uint64_t)blockIdx.x * 256 + threadIdx.x;
-    if (i >= n) return;
-    const uint32_t s = sel[i], r = s & ~MERGE_B;
-    const uint32_t *o = (s & MERGE_B) ? ob : oa;
-    lens[i] = o[r + 1] - o[r];
-}
-
-// MERGE_STR_LANES lanes per output row (short strings: see join_str_copy_kernel)
-constexpr uint32_t MERGE_STR_LANES = 8;
-__global__ void __launch_bounds__(256) merge_str_copy_kernel(const uint8_t *__restrict__ da, const uint32_t *__restrict__ oa, const uint8_t *__restrict__ db,
-                                                             const uint32_t *__restrict__ ob, const uint32_t *__restrict__ sel, uint64_t n,
-                                                             const uint64_t *__restrict__ pos, uint32_t *__restrict__ dst_off, uint8_t *__restrict__ dst) {
-    const uint64_t t = (uint64_t)blockIdx.x * 256 + threadIdx.x;
-    const uint64_t i = t / MERGE_STR_LANES;
-    const uint32_t lane = (uint32_t)(t % MERGE_STR_LANES);
-    if (i > n) return;
-    const uint64_t d0 = pos[i];
-    if (lane == 0) dst_off[i] = (uint32_t)d0;  // entry n = total
-    if (i == n) return;
-    const uint32_t s = sel[i], r = s & ~MERGE_B;
-    const uint8_t *src = (s & MERGE_B) ? db : da;
-    const uint32_t *o = (s & MERGE_B) ? ob : oa;
-    const uint32_t s0 = o[r], len = o[r + 1] - s0;
-    for (uint32_t k = lane; k < len; k += MERGE_STR_LANES) dst[d0 + k] = src[s0 + k];
 }
 
 }  // namespace tplx

@@ -458,6 +458,9 @@ struct tplx_stage {
 static constexpr std::memory_order relaxed = std::memory_order_relaxed;
 
 static size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
+// Allocation size of a buffer of `total` string bytes: a 4-byte multiple, readable up to the next 16-byte boundary and 16 bytes
+// beyond (the memory contract of strops.cuh: its word-wise readers load every aligned word that holds a byte of a string).
+static size_t str_buf_bytes(uint64_t total) { return align_up(total, 16) + 16; }
 
 extern "C" int32_t tplx_gpu_stage_create(const void *desc, uint64_t desc_bytes, tplx_stage **out) {
     if (!desc || !out || desc_bytes < sizeof(tplx_stage_header)) return fail(TPLX_E_BADARG, "stage_create: bad arguments");
@@ -797,7 +800,7 @@ static int32_t stage_dev(tplx_stage *s, Device *d, StageDev **out) {
     size_t nb = std::max<size_t>(dec.size() * sizeof(DInstr), 16);
     CU(cudaMalloc(&sd.prog, nb));
     CU(cudaMemcpy(sd.prog, dec.data(), dec.size() * sizeof(DInstr), cudaMemcpyHostToDevice));
-    CU(cudaMalloc(&sd.cpool, align_up(s->cpool.size(), 16) + 16));  // word-wise readers may touch the padding
+    CU(cudaMalloc(&sd.cpool, str_buf_bytes(s->cpool.size())));
     CU(cudaMemcpy(sd.cpool, s->cpool.data(), s->cpool.size(), cudaMemcpyHostToDevice));
     CU(cudaMalloc(&sd.opids, std::max<size_t>(s->opids.size() * 8, 16)));
     CU(cudaMemcpy(sd.opids, s->opids.data(), s->opids.size() * 8, cudaMemcpyHostToDevice));
@@ -914,7 +917,7 @@ extern "C" int32_t tplx_gpu_block_upload(int32_t device, const tplx_column *cols
         ci.type = cols[c].type;
         uint64_t nb = cols[c].type == TPLX_T_STR ? cols[c].data_bytes : n_rows * 8;
         void *dd = nullptr;
-        CU(cudaMallocAsync(&dd, align_up(nb, 16) + 16, d->copy_stream));  // 4-byte-multiple buffers: strops.cuh memory contract
+        CU(cudaMallocAsync(&dd, str_buf_bytes(nb), d->copy_stream));
         b->owned.push_back(dd);
         if (nb) CU(cudaMemcpyAsync(dd, cols[c].data, nb, cudaMemcpyHostToDevice, d->copy_stream));
         ci.data = dd;
@@ -1403,6 +1406,76 @@ static int32_t dalloc(tplx_result *r, T **p, size_t count) {
     return TPLX_OK;
 }
 
+// lens[0 .. n) = string lengths, in place to their exclusive scan; *total = lens[n], fetched with a synchronise. A total beyond 32-bit
+// offsets fails with `what`.
+static int32_t str_total(Device *d, uint64_t *lens, uint64_t n, uint64_t *total, const char *what) {
+    int32_t rc = device_scan(d, lens, lens, n, true);
+    if (rc) return rc;
+    CU(cudaMemcpyAsync(total, lens + n, 8, cudaMemcpyDeviceToHost, d->stream));
+    CU(cudaStreamSynchronize(d->stream));
+    if (*total > 0xFFFFFFFFull) return fail(TPLX_E_OVERFLOW, what);
+    return TPLX_OK;
+}
+
+// Events of a result made outside stage_run (join probe, merge, hash export), from which tplx_gpu_result_info derives kernel_ms and
+// total_ms: result_begin after the input block `in` (may be null) is ready, result_end when all work is enqueued.
+static int32_t result_begin(tplx_result *r, const tplx_block *in) {
+    Device *d = r->dev;
+    CU(cudaEventCreate(&r->ev0));
+    CU(cudaEventCreate(&r->ev1));
+    CU(cudaEventCreate(&r->evk0));
+    CU(cudaEventCreate(&r->evk1));
+    if (in && in->ready) CU(cudaStreamWaitEvent(d->stream, in->ready, 0));
+    CU(cudaEventRecord(r->ev0, d->stream));
+    CU(cudaEventRecord(r->evk0, d->stream));
+    return TPLX_OK;
+}
+static int32_t result_end(tplx_result *r) {
+    Device *d = r->dev;
+    CU(cudaGetLastError());
+    CU(cudaEventRecord(r->evk1, d->stream));
+    CU(cudaEventRecord(r->ev1, d->stream));
+    CU(cudaStreamSynchronize(d->stream));
+    return TPLX_OK;
+}
+
+// Output column `oc` of r (type r->out_types[oc]) from n rows picked by `sel` out of sources a and b (gather.cuh). A validity bitmap
+// is made when force_valid or a source has one. Launches: 5 for a string column, 1 for fixed width, +1 for a bitmap. `what` is the
+// error message of a string column beyond 4 GiB.
+static int32_t gather_column(tplx_result *r, size_t oc, SelSrc a, SelSrc b, uint32_t b_bit, const uint32_t *sel, uint64_t n, bool force_valid,
+                             const char *what) {
+    Device *d = r->dev;
+    const uint32_t nb = (uint32_t)((n + SEL_NT - 1) / SEL_NT);
+    int32_t rc;
+    if (r->out_types[oc] == TPLX_T_STR) {
+        uint64_t *lens = nullptr, tot = 0;
+        CU(cudaMallocAsync((void **)&lens, (n + 1) * 8, d->stream));
+        if (n) sel_str_len_kernel<<<nb, SEL_NT, 0, d->stream>>>(a, b, b_bit, sel, n, lens);
+        rc = str_total(d, lens, n, &tot, what);
+        if (!rc) rc = dalloc(r, &r->out[oc].offsets, n + 1);
+        if (!rc) rc = dalloc(r, &r->out[oc].bytes, str_buf_bytes(tot));
+        if (!rc)
+            sel_str_copy_kernel<<<(uint32_t)(((n + 1) * SEL_STR_LANES + SEL_NT - 1) / SEL_NT), SEL_NT, 0, d->stream>>>(
+                a, b, b_bit, sel, n, lens, r->out[oc].offsets, r->out[oc].bytes);
+        cudaFreeAsync(lens, d->stream);
+        if (rc) return rc;
+        r->out[oc].cap_bytes = tot;
+        r->str_bytes[oc] = tot;
+        r->launches += 5;
+    } else {
+        if ((rc = dalloc(r, &r->out[oc].data, n))) return rc;
+        if (n) sel_gather_fixed_kernel<<<nb, SEL_NT, 0, d->stream>>>(a, b, b_bit, sel, n, r->out[oc].data);
+        r->launches += 1;
+    }
+    if (force_valid || a.valid || b.valid) {
+        if ((rc = dalloc(r, &r->out_valid[oc], (n + 31) / 32 + 1))) return rc;
+        if (n) sel_gather_valid_kernel<<<nb, SEL_NT, 0, d->stream>>>(a, b, b_bit, sel, n, r->out_valid[oc]);
+        r->launches += 1;
+    }
+    CU(cudaGetLastError());
+    return TPLX_OK;
+}
+
 // K1v (vecvm.cuh): fixed-width stages, vector-at-a-time. Outputs are fixed width, so capacities are exact (n rows) and the only
 // retry is for exception records.
 template <int J>
@@ -1692,7 +1765,7 @@ static int32_t run_rows(tplx_stage *s, StageDev *sd, const tplx_block *b, int64_
                 oc.cap_bytes = cap_bytes[c];
                 rc = dalloc(r, &oc.offsets, cap_rows + 1);
                 if (rc) return rc;
-                rc = dalloc(r, &oc.bytes, align_up(cap_bytes[c], 16) + 16);  // strops.cuh contract: readable to the next 16-byte boundary
+                rc = dalloc(r, &oc.bytes, str_buf_bytes(cap_bytes[c]));
                 if (rc) return rc;
                 oc.data = nullptr;
             } else {
@@ -2003,7 +2076,7 @@ static int32_t run_rows_prefiltered(tplx_stage *s, StageDev *sd, const tplx_bloc
         for (uint32_t k = 0; k < G.n_cols; ++k) {
             if (G.type[k] != TPLX_T_STR) continue;
             if (totals[k] > 0xFFFFFFFFull) { drop_ra(); return fail(TPLX_E_OVERFLOW, "gathered string column exceeds 4 GiB"); }
-            rc = dalloc(r, &G.dst_bytes[k], align_up(totals[k], 16) + 16);
+            rc = dalloc(r, &G.dst_bytes[k], str_buf_bytes(totals[k]));
             if (rc) { drop_ra(); return rc; }
         }
         CU(cudaMemcpyAsync(dG, &G, sizeof(G), cudaMemcpyHostToDevice, d->stream));
