@@ -293,6 +293,18 @@ int32_t tplx_gpu_result_device_validity(tplx_result *res, uint32_t col, const ui
 int32_t tplx_gpu_result_merge_resolved(tplx_result *res, const tplx_block *resolved, const int64_t *resolved_row_nos, int64_t first_row_no,
                                        tplx_result **out);
 
+/* ---- device key sort (K11) ------------------------------------------------------------------ */
+/* The rows of any result (a hash_finish result, a stage result, a join probe, a merge) ordered by its first n_keys visible columns,
+ * as a new result that owns its columns: the same visible columns, n_out_rows rows, no exception records; `res` is unchanged. The
+ * order is the one the Python host path gives groups of one type per column: None first, i64 as signed integers, bool False before
+ * True, str by bytes (a string before any longer string it is a prefix of; for valid UTF-8 this is Python's str order); columns
+ * compare lexicographically, the first most significant; rows with equal keys keep their input order (stable). `col_flags` is
+ * NULL or holds one value per visible column; the only flag it takes is TPLX_CONCAT_DROP_VALID (the caller has counted no None in
+ * that column: the output column gets no bitmap). n_keys of 0 or above TPLX_MAX_KEYS, a key column out of range or another flag:
+ * TPLX_E_BADARG; an f64 key column: TPLX_E_UNSUPPORTED; 2^31 rows or more: TPLX_E_OVERFLOW; a failed device allocation:
+ * TPLX_E_NOMEM, nothing is kept. kernel_ms and kernel_launches of the output's tplx_result_info cover the sort and the gathers. */
+int32_t tplx_gpu_result_sort_by_keys(tplx_result *res, uint32_t n_keys, const uint8_t *col_flags, tplx_result **out);
+
 /* ---- multi-GPU: the one exchange step of the path ------------------------------------------- */
 /* One rank per (process, device) over NCCL (NVLink 5 / NVSwitch). Map / filter stages shard over ranks without any
  * communication (one task per partition group, LocalBackend.cc:679-735); only aggregate endpoints exchange data:

@@ -126,6 +126,7 @@ def lib():
         "tplx_gpu_result_fetch_validity": ([vp, u32, vp, P(u32)], i32),
         "tplx_gpu_result_device_validity": ([vp, u32, P(vp)], i32),
         "tplx_gpu_result_merge_resolved": ([vp, vp, P(i64), i64, P(vp)], i32),
+        "tplx_gpu_result_sort_by_keys": ([vp, u32, ct.c_char_p, P(vp)], i32),
         "tplx_gpu_comm_unique_id": ([vp], i32),
         "tplx_gpu_comm_init": ([i32, i32, i32, vp], i32),
         "tplx_gpu_comm_init_local": ([P(i32), i32], i32),
@@ -701,6 +702,17 @@ class Result:
         _check(lib().tplx_gpu_result_merge_resolved(self._h, resolved._h, arr, first_row_no, ct.byref(h)), "tplx_gpu_result_merge_resolved")
         r = Result(h, None, resolved, types=self.out_types())
         r._rowidx = self.rowidx
+        return r
+
+    def sort_by_keys(self, n_keys: int, col_flags: Optional[Sequence[int]] = None) -> "Result":
+        """The rows ordered by the first `n_keys` columns, stably, None first (K11, tplx_gpu_result_sort_by_keys), as a new result
+        with the same visible columns; `col_flags` holds 0 or CONCAT_DROP_VALID per column (None: 0 for every column)."""
+        h = ct.c_void_p()
+        flags = bytes(col_flags) if col_flags is not None else None
+        _check(lib().tplx_gpu_result_sort_by_keys(self._h, n_keys, flags, ct.byref(h)), "tplx_gpu_result_sort_by_keys")
+        r = Result(h, None, None, types=self.out_types())
+        r._rowidx = self.rowidx
+        r.device = self.device
         return r
 
     def exception_partition(self) -> bytes:

@@ -35,6 +35,7 @@
 #include "merge.cuh"
 #include "concat.cuh"
 #include "cache.cuh"
+#include "sort.cuh"
 #include "jit.inl"
 
 using namespace tplx;
@@ -2426,3 +2427,4 @@ extern "C" int32_t tplx_gpu_result_fetch_aggregate(tplx_result *r, int64_t *acc_
 #include "tplx_gpu_join.inl"
 #include "tplx_gpu_merge.inl"
 #include "tplx_gpu_concat.inl"
+#include "tplx_gpu_sort.inl"

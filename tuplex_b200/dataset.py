@@ -178,11 +178,11 @@ class DeviceSource(Source):
 
 
 class _CachedPart:
-    """One block of a cached dataset as a part of DeviceRows. It reads like a stage result; a consumer that takes it as a block gets
-    a view (as_block), so that freeing its input leaves the cache intact."""
+    """One block of a cached dataset (or of re-blocked groups, which `owns` it) as a part of DeviceRows. It reads like a stage
+    result; a consumer that takes it as a block gets a view (as_block), so that freeing its input leaves the block intact."""
 
-    def __init__(self, block, types: List[int]):
-        self.block, self.types, self.device = block, list(types), block.device
+    def __init__(self, block, types: List[int], owns: bool = False):
+        self.block, self.types, self.device, self.owns = block, list(types), block.device, owns
         n = int(block.n_rows)
         nb = block.column_bytes()
         self.info = _PartInfo(n, [nb[c] - (n + 1) * 4 if t == T_STR else 0 for c, t in enumerate(self.types)])
@@ -197,7 +197,8 @@ class _CachedPart:
         return self.block.validity(c)
 
     def free(self):
-        pass
+        if self.owns:
+            self.block.free()
 
 
 class _PartInfo:
@@ -476,7 +477,8 @@ class DataSet:
         src = self._source
         if isinstance(src, CacheSource) and not self._ops and self._join is None and self._parent is None:
             return DataSet(self._ctx, src)
-        rows, names = self._execute(handoff=_handoff_ok(self._ctx))
+        hash_end = bool(self._ops) and self._ops[-1].kind in ("aggregateByKey", "unique")  # groups are cached on the host path
+        rows, names = self._execute(handoff=_handoff_ok(self._ctx) and not hash_end)
         if isinstance(rows, DeviceRows):
             if rows.n_rows:
                 ds, rows = _device_cache(self._ctx, rows, names)
@@ -599,7 +601,8 @@ class DataSet:
     def _execute(self, csv_sink: Optional[list] = None, csv_null: str = "", handoff: bool = False):
         """Split the operator chain into stages and run them. Returns (python rows, column names). With `csv_sink` (a list) the
         last stage may instead write its rows there as CSV text, None cells as `csv_null`, and return (None, column names). With
-        `handoff` (the consumer is a join) a last row stage may instead return its results on the device, as a DeviceRows."""
+        `handoff` (the consumer is a join or cache()) a last row or hash stage may instead return its results on the device, as a
+        DeviceRows."""
         src = self._source
         self._last_exceptions = Counter()
         if handoff and isinstance(src, CacheSource) and not self._ops and self._parent is None:
@@ -635,10 +638,11 @@ class DataSet:
         rows = names = None
         for si, ops in enumerate(stages):
             if si > 0:
-                src = self._ctx._source_from_rows(rows, names)
+                src = DeviceSource(self._ctx, _reblocked(self._ctx, rows)) if isinstance(rows, DeviceRows) else self._ctx._source_from_rows(rows, names)
             last = si == len(stages) - 1
+            # a stage before the last ends in an endpoint; a hash endpoint then hands its groups to the next stage on the device
             rows, names = _run_stage(self._ctx, src, ops, self._last_exceptions, csv_sink=csv_sink if last else None, csv_null=csv_null,
-                                     handoff=handoff and last)
+                                     handoff=handoff or not last)
         return rows, names
 
 
@@ -1028,7 +1032,8 @@ def _run_stage(ctx, src: Source, ops: List[Op], exc_counter: Counter, csv_sink: 
     elif end.kind == "aggregate":
         rows, names = _aggregate_endpoint(plan, st, src.names, exc_counter)
     else:
-        rows, names = _hash_endpoint(plan, stage, st, list(dict.fromkeys(sh.dev for sh in shards)), src.names, exc_counter)
+        rows, names = _hash_endpoint(plan, stage, st, list(dict.fromkeys(sh.dev for sh in shards)), src.names, exc_counter, ctx, csv_sink,
+                                     csv_null, handoff)
     stage.close()
     return rows, names
 
@@ -1322,16 +1327,36 @@ def _aggregate_endpoint(plan: _StagePlan, st: _Shard, names, exc_counter: Counte
     return [value], [None] * (len(value) if isinstance(value, tuple) else 1)
 
 
-def _hash_endpoint(plan: _StagePlan, stage, st: _Shard, devs: List[int], names, exc_counter: Counter):
+def _hash_endpoint(plan: _StagePlan, stage, st: _Shard, devs: List[int], names, exc_counter: Counter, ctx=None, csv_sink: Optional[list] = None,
+                   csv_null: str = "", handoff: bool = False):
     """Hash endpoint (aggregateByKey, unique): each of `devs` holds the groups it owns after the exchange (a single table
-    otherwise). Rows outside the normal case (other types, CSV rows with nulls / unparsable cells, rows whose UDF raised on
-    the device) are resolved by the interpreter and join the groups like any other row (ResolveTask feeds the same hash sink,
-    core/src/physical/ResolveTask.cc:618-700)."""
+    otherwise). Given the context: on one device, with None kept in the normal case and no row for the interpreter, the groups are ordered on the
+    device (_device_groups) and stay there: with `handoff` they are returned as DeviceRows, with a CSV sink K7 writes them into
+    `csv_sink` (None is returned), else they are fetched in that order. Otherwise rows outside the normal case (other types, CSV rows
+    with nulls / unparsable cells, rows whose UDF raised on the device) are resolved by the interpreter and join the groups like any
+    other row (ResolveTask feeds the same hash sink, core/src/physical/ResolveTask.cc:618-700), and the groups are sorted here."""
     prog, end = plan.prog, plan.end
     nk = prog.n_keys
+    out_names = list(prog.out_names) + [None] * len(prog.accs)
     vals: List[list] = []
+    first = None
+    if ctx is not None and len(devs) == 1 and _handoff_ok(ctx) and not st.interpreter_rows():
+        first = stage.hash_finish(devs[0])
+        first.device = devs[0]
+        groups = _device_groups(first, nk)
+        if groups is not None:
+            rows = DeviceRows([groups], out_names, groups.out_types())
+            if handoff:
+                return rows, out_names
+            chunks = rows.csv(csv_null) if csv_sink is not None else None
+            if chunks is not None:
+                _count_handoff(ctx, rows.n_rows)
+                rows.free()
+                csv_sink.extend(chunks)
+                return None, out_names
+            return rows.rows(), out_names
     for dv in devs:
-        res = stage.hash_finish(dv)
+        res = first if first is not None else stage.hash_finish(dv)
         cols = res.columns()
         res.free()
         part_vals = [c.to_values() for c in cols]
@@ -1368,7 +1393,42 @@ def _hash_endpoint(plan: _StagePlan, stage, st: _Shard, devs: List[int], names, 
         table[key] = list(nv) if isinstance(nv, tuple) else [nv]
     order.sort(key=_key_order)
     rows = [tuple(list(k) + table[k]) if (len(k) + len(table[k])) != 1 else k[0] for k in order]
-    return rows, list(prog.out_names) + [None] * len(prog.accs)
+    return rows, out_names
+
+
+def _device_groups(res, nk: int):
+    """The groups of a hash_finish result in the host path's order (_key_order), sorted on the device by their nk key columns (K11,
+    Result.sort_by_keys), and typed as Context._source_from_rows types the same rows: a column without None loses its bitmap. The
+    sorted result (which frees `res`), or None (res kept) where only the host path gives the answer: no group, an f64 key, a string
+    that is not valid UTF-8 (the host decodes it with "replace", and distinct byte keys may collapse), a column that is None in
+    every group (typed from its values on the host path)."""
+    n = int(res.info.n_out_rows)
+    types = res.out_types()
+    if n == 0 or any(t == T_F64 for t in types[:nk]):
+        return None
+    blk = res.as_block()
+    none, bad = blk.stats()
+    blk.free()
+    if any(bad) or any(k == n for k in none):
+        return None
+    out = res.sort_by_keys(nk, [backend.CONCAT_DROP_VALID if k == 0 else 0 for k in none])
+    res.free()
+    return out
+
+
+def _reblocked(ctx, rows: DeviceRows) -> DeviceRows:
+    """Rows cut at multiples of tuplex.gpu.blockRows, the cut _column_blocks makes over a host source of the same rows (so that
+    an f64 aggregate over them sums the same blocks); rows that fit in one block are returned as they are."""
+    sizes = [int(p.info.n_out_rows) for p in rows.parts]
+    plan = _cache_plan(sizes, ctx._block_rows)
+    if len(plan) <= 1:
+        return rows
+    views = [p.as_block(len(rows.types)) for p in rows.parts]
+    blocks = [backend.Block.concat_pieces([(views[p], f, k) for p, f, k in pieces]) for pieces in plan]
+    for v in views:
+        v.free()
+    rows.free()
+    return DeviceRows([_CachedPart(b, rows.types, owns=True) for b in blocks], rows.names, rows.types)
 
 
 def _acc_value(kind: int, bits: int):
