@@ -12,6 +12,7 @@ them on the CPython path, merge in order.
 from __future__ import annotations
 
 import threading
+import time
 import weakref
 from collections import Counter
 from concurrent.futures import ThreadPoolExecutor
@@ -747,101 +748,121 @@ def _rows_as_tuples(rows):
 
 def _run_join(ctx, spec: JoinSpec, exc_counter: Counter, handoff: bool = False):
     """A JoinOperator between two executed datasets: HashJoinStage of the reference (core/src/physical/HashJoinStage.cc; build stage
-    with a hash-table endpoint + probe inside the other side's pipeline, PipelineBuilder.cc:2110-2523) on the GPU (K8,
-    tplx_gpu_join_build / tplx_gpu_join_probe). Sides that a stage or join left on the device are joined there (_device_join);
-    otherwise every side comes to the host as rows and rows outside the normal case of either side (fallback rows) are joined on
-    the interpreter path and merged by (probe row, build row), which is the order the normal case produces. With `handoff` the
-    output may stay on the device (DeviceRows)."""
+    with a hash-table endpoint + probe inside the other side's pipeline, PipelineBuilder.cc:2110-2523) on the GPU (K8, _join_probes).
+    A side that a stage or join left on the device (DeviceRows) is joined there, unless the host path's typing or merge decides: a
+    column that is None in every row, fallback rows on a host side, key types that differ, or the interpreter path. Rows outside the
+    normal case of either side (fallback rows) are joined on the interpreter path and merged by (probe row, build row), which is the
+    order the normal case produces. With `handoff` the output of a join that took a side from the device stays there (DeviceRows)."""
     ok = _handoff_ok(ctx)
     left, lnames = spec.left._execute(handoff=ok)
     right, rnames = spec.right._execute(handoff=ok)
     exc_counter.update(spec.left._last_exceptions)
     exc_counter.update(spec.right._last_exceptions)
-    lnames = list(lnames) if lnames else []
-    rnames = list(rnames) if rnames else []
-    if ok:
-        out = _device_join(ctx, spec, left, lnames, right, rnames, handoff)
-        if out is not None:
-            return out
-    lrows = left.rows() if isinstance(left, DeviceRows) else left
-    rrows = right.rows() if isinstance(right, DeviceRows) else right
-    li, ri = spec.key_indices(lnames, rnames)
-    names = spec.names(lnames, rnames)
+    nms = [list(lnames) if lnames else [], list(rnames) if rnames else []]
+    li, ri = spec.key_indices(*nms)
+    names = spec.names(*nms)
     build_right = spec.build_right()
     left_outer = spec.kind == "left"
-    lsrc = ctx._source_from_rows(lrows, lnames, option=True)
-    rsrc = ctx._source_from_rows(rrows, rnames, option=True)
-    n_left_cols, n_right_cols = len(lnames), len(rnames)
+    n_left_cols, n_right_cols = len(nms[0]), len(nms[1])
+    sides = [left, right]  # DeviceRows, or Python rows with their host source in srcs
+    srcs = [None if isinstance(s, DeviceRows) else ctx._source_from_rows(s, nm, option=True) for s, nm in zip(sides, nms)]
+
+    def types(i: int) -> List[int]:
+        return sides[i].types if srcs[i] is None else srcs[i].col_types
+
+    def shaped() -> bool:
+        return len(types(0)) == n_left_cols and len(types(1)) == n_right_cols
+
+    def home():
+        for i in (0, 1):
+            if srcs[i] is None:
+                sides[i] = sides[i].rows()
+                srcs[i] = ctx._source_from_rows(sides[i], nms[i], option=True)
 
     def python_join():
         """Interpreter path of the whole join (key types the device does not hash, empty sides)."""
-        L, R = _rows_as_tuples(lrows), _rows_as_tuples(rrows)
+        home()
+        L, R = _rows_as_tuples(sides[0]), _rows_as_tuples(sides[1])
         return _py_join_pairs(L, li, R, ri, left_outer, build_right, n_right_cols), names
 
-    if not lrows or not rrows or len(lsrc.cols) != n_left_cols or len(rsrc.cols) != n_right_cols:
+    if None in srcs and (not ok or not shaped() or types(0)[li] != types(1)[ri] or any(s is not None and s.fallback for s in srcs)
+                         or any(s.none_column() for s in sides if isinstance(s, DeviceRows))):
+        home()
+    if any(s is not None and not rows for s, rows in zip(srcs, sides)) or not shaped():
         return python_join()
-    lk, rk = lsrc.cols[li], rsrc.cols[ri]
-    if lk.type != rk.type:  # a side whose keys are all None takes the other side's key type (NULLVALUE vs Option[T], JoinOperator.cc:121-131)
+    if types(0)[li] != types(1)[ri]:  # both sides are host sources here
+        lk, rk = srcs[0].cols[li], srcs[1].cols[ri]
+        # a side whose keys are all None takes the other side's key type (NULLVALUE vs Option[T], JoinOperator.cc:121-131)
         if rk.valid is not None and not rk.present().any():
-            rsrc.cols[ri] = rk = Column.from_values([None] * len(rk), lk.type)
+            srcs[1].cols[ri] = Column.from_values([None] * len(rk), lk.type)
         elif lk.valid is not None and not lk.present().any():
-            lsrc.cols[li] = lk = Column.from_values([None] * len(lk), rk.type)
+            srcs[0].cols[li] = Column.from_values([None] * len(lk), rk.type)
         else:
             raise TypeError(f"can't perform join, left column '{spec.left_col}' type {ir.TYPE_NAMES[lk.type]} is not the same as right column "
                             f"'{spec.right_col}' type {ir.TYPE_NAMES[rk.type]}")
-    if lk.type == T_F64 or len(names) > C["TPLX_MAX_COLS"] - 2:
+    if types(0)[li] == T_F64 or len(names) > C["TPLX_MAX_COLS"] - 2:
         return python_join()
 
-    need_idx = bool(lsrc.fallback or rsrc.fallback)
-    lcols, rcols = list(lsrc.cols), list(rsrc.cols)
+    need_idx = any(s is not None and s.fallback for s in srcs)  # then both sides are host sources
+    cols = [None if s is None else list(s.cols) for s in srcs]  # per host side: the columns it uploads
     if need_idx:  # original row numbers travel as one more payload column per side: the merge below orders by them
-        lcols.append(Column(T_I64, lsrc.orig_index if lsrc.orig_index is not None else np.arange(lsrc.n_rows, dtype=np.int64)))
-        rcols.append(Column(T_I64, rsrc.orig_index if rsrc.orig_index is not None else np.arange(rsrc.n_rows, dtype=np.int64)))
-    probe_cols, build_cols, pk, bk = (lcols, rcols, li, ri) if build_right else (rcols, lcols, ri, li)
-    n_probe, n_build = (lsrc.n_rows, rsrc.n_rows) if build_right else (rsrc.n_rows, lsrc.n_rows)
-    block_rows = ctx._block_rows
-    blocks = [(lo, min(n_probe, lo + block_rows)) for lo in range(0, n_probe, block_rows)] or [(0, 0)]
-    devs = ctx._devices if len(blocks) > 1 else [ctx._device]  # a single probe block has nothing to shard
-    backend.init(sorted(set(devs)))
+        for c, s in zip(cols, srcs):
+            c.append(Column(T_I64, s.orig_index if s.orig_index is not None else np.arange(s.n_rows, dtype=np.int64)))
+    col_types = [types(i) if cols[i] is None else [c.type for c in cols[i]] for i in (0, 1)]
+    pi, bi = (0, 1) if build_right else (1, 0)
+    pk, bk = (li, ri) if build_right else (ri, li)
 
-    def run_shard(dev: int, dev_blocks):
+    def pieces(i: int) -> list:
+        """Side i's device results, or row ranges of its host columns: the build side whole, the probe side by tuplex.gpu.blockRows."""
+        if cols[i] is None:
+            return sides[i].parts
+        n = srcs[i].n_rows
+        if i == bi:
+            return [(0, n)]
+        return [(lo, min(n, lo + ctx._block_rows)) for lo in range(0, n, ctx._block_rows)] or [(0, 0)]
+
+    def block(i: int, dev: int, piece):
+        if cols[i] is None:
+            return piece.as_block(len(col_types[i]))
+        lo, hi = piece
+        return backend.Block.upload(dev, cols[i] if (lo, hi) == (0, srcs[i].n_rows) else [c.slice(lo, hi) for c in cols[i]], hi - lo)
+
+    device_out = handoff and None in srcs  # one device here (_handoff_ok)
+
+    def task(dev: int, probe_pieces) -> list:
         """One task per device: the table is built once per device (broadcast of the small side), the device's contiguous run of
-        probe blocks goes through it in order; no exchange between devices."""
-        bb = backend.Block.upload(dev, build_cols, n_build)
-        jn = backend.Join(bb, [c.type for c in build_cols], bk)
-        outs = []
-        for lo, hi in dev_blocks:
-            cols = [c.slice(lo, hi) for c in probe_cols] if (lo, hi) != (0, n_probe) else probe_cols
-            pb = backend.Block.upload(dev, cols, hi - lo)
-            res = jn.probe(pb, [c.type for c in probe_cols], pk, left_outer=left_outer, build_first=not build_right)
-            info = res.info
-            with _metrics_lock:
-                ctx.metrics._add(info)
-                ctx.metrics.join_probe_rows = getattr(ctx.metrics, "join_probe_rows", 0) + (hi - lo)
-            outs.append(res.columns())
+        probe blocks goes through it in order; no exchange between devices. Returns the results, or the values of their columns,
+        each result fetched and freed as it comes."""
+        results = _join_probes(ctx, [block(bi, dev, p) for p in pieces(bi)], col_types[bi], bk, (block(pi, dev, p) for p in probe_pieces),
+                               col_types[pi], pk, left_outer, not build_right)
+        if device_out:
+            return list(results)
+        vals: List[list] = [[] for _ in range(len(col_types[0]) + len(col_types[1]) - 1)]
+        for res in results:
+            for acc, col in zip(vals, res.columns()):
+                acc.extend(col.to_values())
             res.free()
-            pb.free()
-        with _metrics_lock:
-            ctx.metrics.join_build_ms = getattr(ctx.metrics, "join_build_ms", 0.0) + jn.info["build_ms"]
-        jn.free()
-        bb.free()
-        return outs
+        return vals
 
-    shard_outs = _per_device(devs, blocks, run_shard)
-    col_vals: Optional[List[list]] = None
-    for outs in shard_outs:
-        for oc in outs:
-            vals = [c.to_values() for c in oc]
-            if col_vals is None:
-                col_vals = vals
-            else:
-                for a, b in zip(col_vals, vals):
-                    a.extend(b)
-    col_vals = col_vals or []
-    n_out = len(col_vals[0]) if col_vals else 0
+    probe_pieces = pieces(pi)
+    devs = ctx._devices if len(probe_pieces) > 1 else [ctx._device]  # a single probe block has nothing to shard
+    backend.init(sorted(set(devs)))
+    on_device = [s for s in sides if isinstance(s, DeviceRows)]
+    for s in on_device:
+        _count_handoff(ctx, s.n_rows)
+    shard_outs = _per_device(devs, probe_pieces, task)
+    for s in on_device:
+        s.free()
+    if device_out:
+        outs = shard_outs[0]
+        return DeviceRows(outs, names, outs[0].out_types() if outs else []), names
+    col_vals = shard_outs[0]
+    for vals in shard_outs[1:]:
+        for a, b in zip(col_vals, vals):
+            a.extend(b)
+    n_out = len(col_vals[0])
     if not need_idx:
-        rows = list(zip(*col_vals)) if len(col_vals) > 1 else list(col_vals[0]) if col_vals else []
-        return rows, names
+        return (list(zip(*col_vals)) if len(col_vals) > 1 else col_vals[0]), names
     # ---- interpreter path for the fallback rows of either side, merged in (probe row, build row) order ----
     # device layout with the index columns: first side's non-key columns (its index last), key, second side's non-key columns (index last)
     left_idx_pos = n_left_cols - 1  # left columns always come first: n_left_cols - 1 non-key payloads, then the index column
@@ -849,9 +870,9 @@ def _run_join(ctx, spec: JoinSpec, exc_counter: Counter, handoff: bool = False):
     lidx, ridx = col_vals[left_idx_pos], col_vals[right_idx_pos]
     keep = [i for i in range(len(col_vals)) if i not in (left_idx_pos, right_idx_pos)]
     gpu_rows = [tuple(col_vals[c][i] for c in keep) for i in range(n_out)]
-    L, R = _rows_as_tuples(lrows), _rows_as_tuples(rrows)
-    lfall = {i for i, _ in lsrc.fallback}
-    rfall = {i for i, _ in rsrc.fallback}
+    L, R = _rows_as_tuples(sides[0]), _rows_as_tuples(sides[1])
+    lfall = {i for i, _ in srcs[0].fallback}
+    rfall = {i for i, _ in srcs[1].fallback}
     extra = _py_join_index_pairs(L, li, R, ri, lfall, rfall)
     merged = {}
     for row, l, r in zip(gpu_rows, lidx, ridx):
@@ -872,83 +893,37 @@ def _run_join(ctx, spec: JoinSpec, exc_counter: Counter, handoff: bool = False):
     return rows, names
 
 
-def _device_join(ctx, spec: JoinSpec, left, lnames, right, rnames, handoff: bool):
-    """The join of two sides of which at least one is on the device (DeviceRows), without bringing it to the host: the build
-    side is one block (a single result wrapped, several concatenated on the device), the probe side's results are probed in
-    order; a host side is uploaded as on the host path. None (nothing run) where only the host path gives the answer: a
-    column that is None in every row, an empty host side, fallback rows on a host side, key types that differ or are f64, too many
-    columns."""
-    sides = [(left, lnames), (right, rnames)]
-    if not any(isinstance(s, DeviceRows) for s, _ in sides):
-        return None
-    li, ri = spec.key_indices(lnames, rnames)
-    names = spec.names(lnames, rnames)
-    types, host_srcs = [], []
-    for s, nm in sides:
-        if isinstance(s, DeviceRows):
-            if s.none_column() or len(s.types) != len(nm):
-                return None
-            types.append(s.types)
-            host_srcs.append(None)
-        else:
-            if not s:
-                return None
-            hs = ctx._source_from_rows(s, nm, option=True)
-            if hs.fallback or len(hs.cols) != len(nm):
-                return None
-            types.append(hs.col_types)
-            host_srcs.append(hs)
-    if types[0][li] != types[1][ri] or types[0][li] == T_F64 or len(names) > C["TPLX_MAX_COLS"] - 2:
-        return None
-    build_right = spec.build_right()
-    left_outer = spec.kind == "left"
-    dev = next(s.device for s, _ in sides if isinstance(s, DeviceRows))
-    backend.init([dev])
-    pi, bi = (0, 1) if build_right else (1, 0)
-    pk, bk = (li, ri) if build_right else (ri, li)
-
-    def blocks(i: int, one: bool) -> list:
-        """Side i as device blocks in row order: its results wrapped, or its host columns uploaded (one block, or blocks of
-        tuplex.gpu.blockRows rows)."""
-        s, hs = sides[i][0], host_srcs[i]
-        if hs is None:
-            return [p.as_block(len(s.types)) for p in s.parts]
-        n, step = hs.n_rows, (hs.n_rows if one else ctx._block_rows)
-        return [backend.Block.upload(dev, [c.slice(lo, min(n, lo + step)) for c in hs.cols], min(n, lo + step) - lo) for lo in range(0, n, step)]
-
-    for s, _ in sides:
-        if isinstance(s, DeviceRows):
-            _count_handoff(ctx, s.n_rows)
-    bparts = blocks(bi, True)
-    if len(bparts) == 1:
-        bb = bparts[0]
-    else:
-        import time
-        t0 = time.perf_counter()
-        bb = backend.Block.concat(bparts)
+def _join_probes(ctx, build: list, build_types: List[int], build_key: int, probe, probe_types: List[int], probe_key: int,
+                 left_outer: bool, build_first: bool):
+    """K8 over blocks of one device: the table is built over the `build` blocks (concatenated on the device when there are several)
+    and every block of `probe` is probed through it in order. Yields one backend.Result per probe block and frees every block it was
+    given; the table and the build block are freed also when an error ends the join."""
+    t0 = time.perf_counter()
+    bb = build[0] if len(build) == 1 else backend.Block.concat(build)
+    if len(build) != 1:
+        ms = (time.perf_counter() - t0) * 1e3
         with _metrics_lock:
-            ctx.metrics.join_concat_ms = getattr(ctx.metrics, "join_concat_ms", 0.0) + (time.perf_counter() - t0) * 1e3
-            ctx.metrics.join_concat_bytes = getattr(ctx.metrics, "join_concat_bytes", 0) + sum(
-                int(p.info.n_out_rows) * 8 if t != T_STR else int(p.info.out_str_bytes[c]) + int(p.info.n_out_rows) * 4
-                for p in sides[bi][0].parts for c, t in enumerate(types[bi]))
-        del bparts
-    jn = backend.Join(bb, types[bi], bk)
-    outs = []
-    for pb in blocks(pi, False):
-        res = jn.probe(pb, types[pi], pk, left_outer=left_outer, build_first=not build_right)
+            ctx.metrics.join_concat_ms = getattr(ctx.metrics, "join_concat_ms", 0.0) + ms
+            ctx.metrics.join_concat_bytes = getattr(ctx.metrics, "join_concat_bytes", 0) + sum(  # n offsets per string column of a part
+                nb - 4 if t == T_STR else nb for b in build for nb, t in zip(b.column_bytes(), build_types))
+        for b in build:
+            b.free()
+    jn = None
+    try:
+        jn = backend.Join(bb, build_types, build_key)
+        for pb in probe:
+            res = jn.probe(pb, probe_types, probe_key, left_outer=left_outer, build_first=build_first)
+            with _metrics_lock:
+                ctx.metrics._add(res.info)
+                ctx.metrics.join_probe_rows = getattr(ctx.metrics, "join_probe_rows", 0) + pb.n_rows
+            yield res
+            pb.free()
         with _metrics_lock:
-            ctx.metrics._add(res.info)
-            ctx.metrics.join_probe_rows = getattr(ctx.metrics, "join_probe_rows", 0) + pb.n_rows
-        outs.append(res)
-    with _metrics_lock:
-        ctx.metrics.join_build_ms = getattr(ctx.metrics, "join_build_ms", 0.0) + jn.info["build_ms"]
-    jn.free()
-    bb.free()
-    for s, _ in sides:
-        if isinstance(s, DeviceRows):
-            s.free()
-    out = DeviceRows(outs, names, outs[0].out_types() if outs else [])
-    return (out if handoff else out.rows()), names
+            ctx.metrics.join_build_ms = getattr(ctx.metrics, "join_build_ms", 0.0) + jn.info["build_ms"]
+    finally:
+        if jn is not None:
+            jn.free()
+        bb.free()
 
 
 def _join_row(lrow, li, rrow, ri, n_right_cols):
