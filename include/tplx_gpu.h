@@ -186,6 +186,17 @@ int32_t tplx_gpu_block_fetch_column(const tplx_block *block, uint32_t col, void 
 /* A block over the same device memory as `block` that owns none of it (freeing it frees nothing of `block`); `block` must
  * outlive it. Lets a block that several consumers read (a cached dataset) go where the consumer frees its input block. */
 int32_t tplx_gpu_block_view(const tplx_block *block, tplx_block **out);
+/* The rows of a device-resident block whose bit is set in `keep_words` (bit r & 31 of word r >> 5, (n_rows + 31) / 32 host words; bits
+ * past n_rows are ignored), in order, as one new block that owns its memory: every column, string offsets rebased, validity bitmaps
+ * realigned (tail bits zero). Built from the stage kernels' survivor list (mask_count / mask_scan / mask_expand) and the row-selector
+ * gathers of join and merge outputs. 2^32 - 1 rows or more: TPLX_E_OVERFLOW. `block` may be freed when the call returns. This is how
+ * a CPython UDF between two device segments of a stage drops rows from the device blocks. */
+int32_t tplx_gpu_block_select(const tplx_block *block, const uint32_t *keep_words, tplx_block **out);
+/* Device addresses of column `col` of a device-resident block, as tplx_gpu_block_wrap_device takes them: values or string bytes,
+ * string offsets (NULL for fixed width), validity bitmap (NULL without one) and the column's data_bytes; waits for the block's
+ * upload. The block must outlive whatever uses them. */
+int32_t tplx_gpu_block_device_column(const tplx_block *block, uint32_t col, const void **data, const uint32_t **offsets,
+                                     const uint32_t **valid, uint64_t *data_bytes);
 
 /* ---- execution -------------------------------------------------------------------------- */
 /* Run the stage over one block (asynchronously on the device's stream; results are complete

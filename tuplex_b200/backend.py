@@ -102,6 +102,8 @@ def lib():
         "tplx_gpu_block_stats": ([vp, P(u64), P(u64)], i32),
         "tplx_gpu_block_fetch_column": ([vp, u32, vp, vp], i32),
         "tplx_gpu_block_view": ([vp, P(vp)], i32),
+        "tplx_gpu_block_select": ([vp, vp, P(vp)], i32),
+        "tplx_gpu_block_device_column": ([vp, u32, P(vp), P(vp), P(vp), P(u64)], i32),
         "tplx_gpu_stage_run": ([vp, vp, i64, P(vp)], i32),
         "tplx_gpu_stage_run_host": ([vp, i32, P(CColumn), u32, u64, i64, P(vp)], i32),
         "tplx_gpu_result_info": ([vp, P(CResultInfo)], i32),
@@ -522,6 +524,25 @@ class Block:
         h = ct.c_void_p()
         _check(lib().tplx_gpu_block_view(self._h, ct.byref(h)), "tplx_gpu_block_view")
         return Block(h, self.n_rows, self.device, keep=self)
+
+    def select(self, keep_words: np.ndarray) -> "Block":
+        """The rows whose bit is set in `keep_words` (bit r & 31 of word r >> 5), in order, as a new block that owns its memory
+        (tplx_gpu_block_select); this block may be freed afterwards."""
+        words = np.ascontiguousarray(keep_words, dtype=np.uint32)
+        if len(words) != (int(self.n_rows) + 31) // 32:
+            raise ValueError("select: one keep word per 32 rows")
+        h = ct.c_void_p()
+        _check(lib().tplx_gpu_block_select(self._h, words.ctypes.data if len(words) else None, ct.byref(h)), "tplx_gpu_block_select")
+        nr = ct.c_uint64()
+        _check(lib().tplx_gpu_block_rows(h, ct.byref(nr)), "tplx_gpu_block_rows")
+        return Block(h, nr.value, self.device)
+
+    def device_column(self, c: int, t: int) -> tuple:
+        """Column c (of type t) as Block.wrap_device takes it: (type, data, offsets, data_bytes, validity), device addresses
+        (tplx_gpu_block_device_column); this block must outlive their use."""
+        d, o, v, nb = ct.c_void_p(), ct.c_void_p(), ct.c_void_p(), ct.c_uint64()
+        _check(lib().tplx_gpu_block_device_column(self._h, c, ct.byref(d), ct.byref(o), ct.byref(v), ct.byref(nb)), "tplx_gpu_block_device_column")
+        return t, d.value or 0, o.value or 0, int(nb.value), v.value or 0
 
     @staticmethod
     def from_partitions(device: int, partitions: Sequence[bytes], col_types: Sequence[int], option_cols: Sequence[int] = ()) -> "Block":

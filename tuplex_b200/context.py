@@ -47,6 +47,23 @@ def _kind(v) -> Optional[int]:
     return None
 
 
+def column_type(values) -> Optional[int]:
+    """Normal-case type of one column: the majority type of its values (PythonContext::inferType), None when no value has one
+    (every value None, or outside the types a column holds)."""
+    cnt = Counter(_kind(v) for v in values)
+    return next((k for k, _ in cnt.most_common() if k is not None), None)
+
+
+def typed_column(values: Sequence) -> Optional[Column]:
+    """The values as one column typed like a column of Context._source_from_rows (Option[T] where some are None), or None where
+    that source would leave rows outside the normal case: a value of another type (an int beyond i64 included), or None in
+    every row."""
+    t = column_type(values)
+    if t is None or any(v is not None and _kind(v) != t for v in values):
+        return None
+    return Column.from_values(values, t)
+
+
 class Metrics:
     """ctx.metrics (tuplex/python/tuplex/metrics.py; JobMetrics.h): counters of the GPU path."""
 
@@ -61,6 +78,8 @@ class Metrics:
         self.device_handoff_rows = 0  # rows passed from one operator to the next as device blocks (join sides and outputs)
         self.cache_rows = 0   # rows cache() placed in device blocks
         self.cache_bytes = 0  # device bytes the cached datasets hold now (falls when a cache is freed)
+        self.split_stages = 0        # stages that ran as device segments around operators whose UDF only CPython runs
+        self.interpreter_values = 0  # values such an operator read column-wise (one per row and column its UDF reads)
 
     def _add(self, info):
         self.rows_in += int(info.n_in_rows)
@@ -140,17 +159,9 @@ class Context:
         # majority type per column (PythonContext::inferType)
         col_types = []
         for c in range(ncols):
-            cnt = Counter()
-            for r in rows:
-                if (len(r) if isinstance(r, tuple) else -1) != arity:
-                    continue
-                v = r[c] if arity != -1 else r
-                cnt[_kind(v)] += 1
-            t = next((k for k, _ in cnt.most_common() if k is not None), None)
-            if t is None:
-                t = T_I64
+            t = column_type(r[c] if arity != -1 else r for r in rows if (len(r) if isinstance(r, tuple) else -1) == arity)
             # ints and bools mixed with floats: keep the majority, the others become fallback rows
-            col_types.append(t)
+            col_types.append(T_I64 if t is None else t)
         normal_vals: List[list] = [[] for _ in range(ncols)]
         orig: List[int] = []
         fallback = []

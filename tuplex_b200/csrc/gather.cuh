@@ -157,4 +157,12 @@ __global__ void __launch_bounds__(SEL_NT) sel_str_copy_kernel(SelSrc a, SelSrc b
     for (uint32_t k = sub; k < len; k += SEL_STR_LANES) dst[d0 + k] = __ldg(bytes + s0 + k);
 }
 
+// survivor list (mask_expand_kernel writes u64 row numbers) -> u32 selectors of the kernels above (tplx_gpu_block_select). The
+// gathers take 32-bit selectors because the merge and join mark the second source in the top bit; mask.cuh's list stays 64-bit
+// for the stage kernels that share it.
+__global__ void __launch_bounds__(SEL_NT) sel_from_rows_kernel(const uint64_t *__restrict__ rows, uint64_t n, uint32_t *__restrict__ sel) {
+    const uint64_t i = (uint64_t)blockIdx.x * SEL_NT + threadIdx.x;
+    if (i < n) sel[i] = (uint32_t)rows[i];
+}
+
 }  // namespace tplx

@@ -197,6 +197,10 @@ class _CachedPart:
     def validity(self, c: int):
         return self.block.validity(c)
 
+    def csv_bytes(self, n_cols: int = 0, null_value: Optional[str] = None):
+        """None: K7 writes stage results, so DeviceRows.csv's caller writes a block's rows with the host writer."""
+        return None
+
     def free(self):
         if self.owns:
             self.block.free()
@@ -338,6 +342,20 @@ def _handoff_ok(ctx) -> bool:
 def _count_handoff(ctx, n: int):
     with _metrics_lock:
         ctx.metrics.device_handoff_rows += int(n)
+
+
+def _deliver(ctx, rows: DeviceRows, names, csv_sink: Optional[list], csv_null: str, handoff: bool):
+    """The last operator's rows on the device to their consumer: as they are with `handoff`, as CSV text written by K7 into
+    `csv_sink` (None returned) when every part can be written there, else as Python rows."""
+    if handoff:
+        return rows, names
+    chunks = rows.csv(csv_null) if csv_sink is not None else None
+    if chunks is not None:
+        _count_handoff(ctx, rows.n_rows)
+        rows.free()
+        csv_sink.extend(chunks)
+        return None, names
+    return rows.rows(), names
 
 
 class JoinSpec:
@@ -612,15 +630,7 @@ class DataSet:
             rows, names = _run_join(self._ctx, self._join, self._last_exceptions, handoff or csv_sink is not None or bool(self._ops))
             if isinstance(rows, DeviceRows):
                 if not self._ops:
-                    if handoff:
-                        return rows, names
-                    chunks = rows.csv(csv_null) if csv_sink is not None else None
-                    if chunks is not None:
-                        _count_handoff(self._ctx, rows.n_rows)
-                        rows.free()
-                        csv_sink.extend(chunks)
-                        return None, names
-                    return rows.rows(), names
+                    return _deliver(self._ctx, rows, names, csv_sink, csv_null, handoff)
                 if rows.none_column():
                     rows = rows.rows()
             if not self._ops:
@@ -710,21 +720,25 @@ def _compile_row_ops(src: Source, ops: Sequence[Op]) -> StageCompiler:
     for any operator that is not a row operator."""
     sc = StageCompiler(src.col_types, src.names, src.option_cols)
     for op in ops:
-        if op.kind == "map":
-            sc.add_map(op.udf, op.id)
-        elif op.kind == "filter":
-            sc.add_filter(op.udf, op.id)
-        elif op.kind == "withColumn":
-            sc.add_with_column(op.column, op.udf, op.id)
-        elif op.kind == "mapColumn":
-            sc.add_map_column(op.column, op.udf, op.id)
-        elif op.kind == "selectColumns":
-            sc.add_select(op.columns, op.id)
-        elif op.kind == "renameColumn":
-            sc.add_rename(op.column, op.extra, op.id)
-        else:
-            raise UnsupportedUDF(f"{op.kind} is not a row operator")
+        _add_row_op(sc, op)
     return sc
+
+
+def _add_row_op(sc: StageCompiler, op: Op):
+    if op.kind == "map":
+        sc.add_map(op.udf, op.id)
+    elif op.kind == "filter":
+        sc.add_filter(op.udf, op.id)
+    elif op.kind == "withColumn":
+        sc.add_with_column(op.column, op.udf, op.id)
+    elif op.kind == "mapColumn":
+        sc.add_map_column(op.column, op.udf, op.id)
+    elif op.kind == "selectColumns":
+        sc.add_select(op.columns, op.id)
+    elif op.kind == "renameColumn":
+        sc.add_rename(op.column, op.extra, op.id)
+    else:
+        raise UnsupportedUDF(f"{op.kind} is not a row operator")
 
 
 def _per_device(devs: List[int], blocks: list, fn) -> list:
@@ -992,6 +1006,9 @@ def _run_stage(ctx, src: Source, ops: List[Op], exc_counter: Counter, csv_sink: 
     try:
         plan = _compile_stage(src, row_ops, end)
     except UnsupportedUDF as e:
+        k = _split_point(ctx, src, row_ops)
+        if k is not None:
+            return _run_split(ctx, src, ops, k, exc_counter, csv_sink, csv_null, handoff)
         ctx._log(f"stage falls back to the CPython path: {e}")
         return _run_stage_python(src.to_host_source(), ops, exc_counter)
     backend.init(sorted(set(ctx._devices)))
@@ -1320,16 +1337,7 @@ def _hash_endpoint(plan: _StagePlan, stage, st: _Shard, devs: List[int], names, 
         first.device = devs[0]
         groups = _device_groups(first, nk)
         if groups is not None:
-            rows = DeviceRows([groups], out_names, groups.out_types())
-            if handoff:
-                return rows, out_names
-            chunks = rows.csv(csv_null) if csv_sink is not None else None
-            if chunks is not None:
-                _count_handoff(ctx, rows.n_rows)
-                rows.free()
-                csv_sink.extend(chunks)
-                return None, out_names
-            return rows.rows(), out_names
+            return _deliver(ctx, DeviceRows([groups], out_names, groups.out_types()), out_names, csv_sink, csv_null, handoff)
     for dv in devs:
         res = first if first is not None else stage.hash_finish(dv)
         cols = res.columns()
@@ -1443,8 +1451,13 @@ def _acc_combine(kind: int, a, b):
 def _run_py(row_ops: Sequence[Op], obj, names, exc_counter: Counter, default_op: int):
     """One row through `row_ops` on the CPython path: (value, names), or None when the row was dropped or raised. A raise stays an
     exception, counted like the reference's exception_counts under the operator that raised (`default_op` when not tagged)."""
+    return _counted(exc_counter, default_op, pyexec.run_row, row_ops, obj, names)
+
+
+def _counted(exc_counter: Counter, default_op: int, fn, *args):
+    """fn(*args), or None when it dropped the row (Dropped) or raised: a raise is counted under the operator it is tagged with."""
     try:
-        return pyexec.run_row(row_ops, obj, names)
+        return fn(*args)
     except Dropped:
         return None
     except Exception as ex:  # noqa: BLE001
@@ -1552,6 +1565,245 @@ def _merge_by_rowno(normal_rows: list, excs: np.ndarray, resolved: List[Tuple[in
         pos += 1
     out.extend(normal_rows[ni:])
     return out
+
+
+# ---- stages split at the operators the device cannot compile -------------------------------------------------------------------
+_ROW_KINDS = ("map", "filter", "withColumn", "mapColumn")
+
+
+def _split_point(ctx, src: Source, row_ops: List[Op]) -> Optional[int]:
+    """Where a stage that does not compile as a whole runs as device segments around one CPython operator U: the position of the
+    first row operator the stage compiler rejects, fed one at a time. U's output stays on the device only on one device with None
+    kept in the normal case (_handoff_ok) over a source without fallback rows, so the split is taken only there, and only when a
+    device segment (the operators before U, or those after it) holds a row operator. None: the whole stage runs in CPython."""
+    if not _handoff_ok(ctx) or src.fallback:
+        return None
+    try:
+        sc = StageCompiler(src.col_types, src.names, src.option_cols)
+    except UnsupportedUDF:
+        return None
+    for k, op in enumerate(row_ops):
+        try:
+            _add_row_op(sc, op)
+        except UnsupportedUDF:
+            if any(o.kind in _ROW_KINDS for i, o in enumerate(row_ops) if i != k):
+                return k
+            return None
+    return None
+
+
+def _run_split(ctx, src: Source, ops: List[Op], k: int, exc_counter: Counter, csv_sink: Optional[list], csv_null: str, handoff: bool):
+    """A stage whose row operator ops[k] (U) only CPython runs: the operators before it run as a device stage over the source (the
+    file parse included) and hand their rows over on the device; U runs in CPython (_interpreter_op); the operators after it, the
+    endpoint included, run as a stage of their own over U's output, split again where they need to be. Rows, their order and
+    exception counts are those of the whole stage on the CPython path."""
+    op = ops[k]
+    ctx._log(f"stage splits at {op.kind} operator {op.id}: its UDF runs in CPython, the operators around it on the device")
+    with _metrics_lock:
+        ctx.metrics.split_stages += 1
+    rows, names = _run_stage(ctx, src, ops[:k], exc_counter, handoff=True)
+    if isinstance(rows, DeviceRows) and rows.n_rows == 0:
+        rows = rows.rows()
+    rows, names = _interpreter_op(ctx, rows, names, op, exc_counter)
+    rest = ops[k + 1:]
+    if isinstance(rows, DeviceRows):
+        if not rest:
+            return _deliver(ctx, rows, names, csv_sink, csv_null, handoff)
+        if rows.none_column():
+            rows = rows.rows()
+    if not isinstance(rows, DeviceRows):
+        if not rows:
+            return _run_stage_python(Source([], names, 0, None, [], 0), rest, exc_counter)
+        if not rest:
+            return rows, names
+    nsrc = DeviceSource(ctx, _reblocked(ctx, rows)) if isinstance(rows, DeviceRows) else ctx._source_from_rows(rows, names)
+    return _run_stage(ctx, nsrc, rest, exc_counter, csv_sink=csv_sink, csv_null=csv_null, handoff=handoff)
+
+
+def _interpreter_op(ctx, rows, names, op: Op, exc_counter: Counter):
+    """U over the rows the device segment before it produced: column-wise over device rows (_columnwise_op) where it can, else
+    row by row over the fetched rows. (rows, names): DeviceRows, or Python rows."""
+    if isinstance(rows, DeviceRows) and op.kind != "map":
+        out = _columnwise_op(ctx, rows, op, exc_counter)
+        if out is not None:
+            return out, out.names
+    if isinstance(rows, DeviceRows):
+        rows = rows.rows()
+    out = [r for r in (_run_py([op], v, names, exc_counter, op.id) for v in rows) if r is not None]
+    if out:
+        return [v for v, _ in out], out[-1][1]
+    if op.kind == "withColumn" and op.column not in names:
+        return rows[:0], list(names) + [op.column]
+    return rows[:0], (_map_output_names(op.udf, names) if op.kind == "map" else list(names))
+
+
+def _columnwise_op(ctx, rows: DeviceRows, op: Op, exc_counter: Counter) -> Optional[DeviceRows]:
+    """A filter / withColumn / mapColumn in CPython over device rows, reading only the columns its UDF and resolvers read
+    (_read_set): each row is called as the row path calls it (pyexec.call_op), the columns it does not read hold None. Dropped rows
+    leave the blocks through tplx_gpu_block_select; a new column is typed as Context._source_from_rows types a column, uploaded and
+    put beside the untouched device columns. None (nothing consumed, nothing counted) when the new values do not make one column
+    (mixed types, an int beyond i64, None in every row) or the target column does not exist: the row path then runs U."""
+    from .context import typed_column
+    names, types = list(rows.names), list(rows.types)
+    ncols = len(types)
+    target = None
+    if op.kind == "mapColumn":
+        if isinstance(op.column, str):
+            if op.column not in names:
+                return None
+            target = names.index(op.column)
+        elif -ncols <= op.column < ncols:
+            target = op.column % ncols
+        else:
+            return None
+    elif op.kind == "withColumn":
+        target = names.index(op.column) if op.column in names else ncols
+    reads = [target] if op.kind == "mapColumn" else _read_set(op, names, ncols)
+
+    def call(value):
+        v = pyexec.call_op(op, value, names)
+        return (bool(v),) if op.kind == "filter" else (v,)
+
+    counts: Counter = Counter()
+    keeps, values = [], []
+    for part in rows.parts:
+        n = int(part.info.n_out_rows)
+        cols = {c: part.column(c).to_values() for c in reads}
+        empty = [None] * n
+        by_col = [cols.get(c, empty) for c in range(ncols)]
+        keep = np.zeros(n, dtype=bool)
+        vals = []
+        for i in range(n):
+            row = tuple(col[i] for col in by_col)
+            r = _counted(counts, op.id, call, row if ncols != 1 else row[0])
+            if r is None or (op.kind == "filter" and not r[0]):
+                continue
+            keep[i] = True
+            vals.append(r[0])
+        keeps.append(keep)
+        values.append(vals)
+    col = None
+    if target is not None:
+        col = typed_column([v for vals in values for v in vals])
+        if col is None:
+            return None
+    exc_counter.update(counts)
+    with _metrics_lock:
+        ctx.metrics.interpreter_values += rows.n_rows * len(reads)
+    out_names, out_types = names, types
+    if target is not None:
+        out_names = names + [op.column] if target == ncols else names
+        out_types = types + [col.type] if target == ncols else types[:target] + [col.type] + types[target + 1:]
+    parts, lo = [], 0
+    for part, keep in zip(rows.parts, keeps):
+        kept = int(keep.sum())
+        parts.append(_spliced(part, ncols, types, keep, None if col is None else col.slice(lo, lo + kept), target, out_types))
+        lo += kept
+    rows.parts = []  # each part now belongs to its successor
+    return DeviceRows(parts, out_names, out_types)
+
+
+class _SplicedPart(_CachedPart):
+    """A part whose block wraps device columns owned by `deps` (freed with it): the columns of an earlier part, with some of its
+    rows selected or not, beside a column uploaded from CPython values."""
+
+    def __init__(self, block, types: List[int], deps: list):
+        super().__init__(block, types, owns=True)
+        self.deps = deps
+
+    def free(self):
+        super().free()
+        for d in self.deps:
+            d.free()
+        self.deps = []
+
+
+def _spliced(part, ncols: int, types: List[int], keep: np.ndarray, col: Optional[Column], target: Optional[int], out_types: List[int]):
+    """`part` with the rows `keep` marks (a select on the device only when one is dropped) and `col` at column `target` (replacing
+    it, or appended when target == ncols). The part is consumed."""
+    if keep.all() and col is None:
+        return part
+    base = part.as_block(ncols)
+    deps = [part]
+    if not keep.all():
+        sel = base.select(backend.pack_valid(keep))
+        base.free()
+        part.free()
+        base, deps = sel, []
+    if col is None:
+        return _SplicedPart(base, out_types, deps)
+    up = backend.Block.upload(base.device, [col], len(col))
+    cols = [base.device_column(c, types[c]) for c in range(ncols)]
+    if target == ncols:
+        cols.append(up.device_column(0, col.type))
+    else:
+        cols[target] = up.device_column(0, col.type)
+    return _SplicedPart(backend.Block.wrap_device(base.device, cols, len(col)), out_types, [base, up] + deps)
+
+
+def _read_set(op: Op, names: List[Optional[str]], ncols: int) -> List[int]:
+    """Columns a filter's or withColumn's UDF and its resolvers read from the row (all of them where the analysis cannot tell)."""
+    cols: set = set()
+    for f in [op.udf] + [r for _, r in op.resolvers]:
+        c = _udf_reads(f, names, ncols)
+        if c is None:
+            return list(range(ncols))
+        cols |= c
+    return sorted(cols)
+
+
+def _udf_reads(udf, names: List[Optional[str]], ncols: int) -> Optional[set]:
+    """The columns a UDF reads from its one row parameter: every use of the parameter must be a subscript by a constant column
+    name or index (negative indices count from the end). None (every column) for a UDF of several parameters (they unpack the
+    row), a row of one column (the parameter is the value), a UDF whose source is not available, and any other use of the row:
+    passed on, iterated, rebound, shadowed."""
+    import ast as _ast
+    from .frontend import get_udf_ast
+    if ncols == 1:
+        return None
+    try:
+        params, body, _ = get_udf_ast(udf)
+    except Exception:  # noqa: BLE001 — the analysis gives up, it does not fail the stage
+        return None
+    if len(params) != 1:
+        return None
+    p = params[0]
+    roots = body if isinstance(body, list) else [body]
+    parent = {}
+    for root in roots:
+        for node in _ast.walk(root):
+            for ch in _ast.iter_child_nodes(node):
+                parent[id(ch)] = node
+    cols = set()
+    for root in roots:
+        for node in _ast.walk(root):
+            if isinstance(node, _ast.arg) and node.arg == p:
+                return None
+            if not (isinstance(node, _ast.Name) and node.id == p):
+                continue
+            sub = parent.get(id(node))
+            if not (isinstance(node.ctx, _ast.Load) and isinstance(sub, _ast.Subscript) and sub.value is node and isinstance(sub.ctx, _ast.Load)):
+                return None
+            c = _const_column(sub.slice, names, ncols)
+            if c is None:
+                return None
+            cols.add(c)
+    return cols
+
+
+def _const_column(key, names: List[Optional[str]], ncols: int) -> Optional[int]:
+    import ast as _ast
+    sign = 1
+    if isinstance(key, _ast.UnaryOp) and isinstance(key.op, _ast.USub):
+        key, sign = key.operand, -1
+    if not isinstance(key, _ast.Constant):
+        return None
+    v = key.value
+    if isinstance(v, str) and sign == 1:
+        return names.index(v) if v in names else None
+    if isinstance(v, int) and not isinstance(v, bool) and -ncols <= sign * v < ncols:
+        return (sign * v) % ncols
+    return None
 
 
 def _run_stage_python(src: Source, ops: List[Op], exc_counter: Counter):

@@ -118,6 +118,16 @@ def _apply_with_resolvers(op: Op, fn):
         raise
 
 
+def call_op(op: Op, value, names: List[Optional[str]]):
+    """What one row gives the UDF of a map / filter / withColumn / mapColumn operator, with its resolvers and ignores applied: the
+    map's result, the filter's verdict, the new column's value. Raises Dropped (an ignored class) or the UDF's exception."""
+    if op.kind == "mapColumn":
+        vals = list(value) if isinstance(value, tuple) else [value]
+        i = names.index(op.column) if isinstance(op.column, str) else op.column
+        return _apply_with_resolvers(op, lambda f: (udf_from_source(f) if isinstance(f, str) else f)(vals[i]))
+    return _apply_with_resolvers(op, lambda f: _call(f, value, names))
+
+
 def run_row(ops: Sequence[Op], value, names: List[Optional[str]]):
     """Run one row through the operator chain in CPython.
     Returns (value, names) or raises: Dropped (filtered / ignored) or the UDF's exception (annotated with .tplx_op)."""
@@ -125,7 +135,7 @@ def run_row(ops: Sequence[Op], value, names: List[Optional[str]]):
     for op in ops:
         try:
             if op.kind == "map":
-                res = _apply_with_resolvers(op, lambda f: _call(f, value, names))
+                res = call_op(op, value, names)
                 if isinstance(res, dict):
                     names = list(res.keys())
                     res = tuple(res.values())
@@ -137,11 +147,11 @@ def run_row(ops: Sequence[Op], value, names: List[Optional[str]]):
                     names = [None]
                     value = res
             elif op.kind == "filter":
-                keep = _apply_with_resolvers(op, lambda f: _call(f, value, names))
+                keep = call_op(op, value, names)
                 if not keep:
                     raise Dropped()
             elif op.kind == "withColumn":
-                res = _apply_with_resolvers(op, lambda f: _call(f, value, names))
+                res = call_op(op, value, names)
                 vals = list(value) if isinstance(value, tuple) else [value]
                 if op.column in names:
                     vals[names.index(op.column)] = res
@@ -151,8 +161,7 @@ def run_row(ops: Sequence[Op], value, names: List[Optional[str]]):
                 value = tuple(vals) if len(vals) != 1 else vals[0]
             elif op.kind == "mapColumn":
                 vals = list(value) if isinstance(value, tuple) else [value]
-                i = names.index(op.column) if isinstance(op.column, str) else op.column
-                vals[i] = _apply_with_resolvers(op, lambda f: (udf_from_source(f) if isinstance(f, str) else f)(vals[i]))
+                vals[names.index(op.column) if isinstance(op.column, str) else op.column] = call_op(op, value, names)
                 value = tuple(vals) if len(vals) != 1 else vals[0]
             elif op.kind == "selectColumns":
                 vals = list(value) if isinstance(value, tuple) else [value]
